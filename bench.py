@@ -1,12 +1,15 @@
 #!/usr/bin/env python
-"""bench.py -- images/sec/GPU of the InstanceDiffusion sampling hot path on B200.
+"""bench.py -- images/sec/GPU of the InstanceDiffusion sampling hot path on H100.
 
 Workload (BASELINE.json configs[1]): batch=4 images of 512x512 (latent 64x64), 8 box instances
 each, 50-step PLMS, classifier-free guidance 7.5, alpha schedule [0.8, 0, 0.2], fp16 compute.
 One "step" of the bench contract = one full `sampler.sample(...)` call over one batch (latent out);
 timed region = the sampler only (no CLIP, no VAE), as SURVEY.md section 8d prescribes.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--mis 0.0] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--mis 0.0] [--impl reference] [--dump-outputs DIR]
+
+--dump-outputs DIR writes the latents the last timed step returned as DIR/latent.npy (float32); weights and
+inputs are seeded, so two builds run with the same arguments can be compared output for output.
 
 N > 1: launched under torch.distributed.run, one rank per GPU; rank 0's synthetic weights are
 broadcast once over NCCL, every rank then samples its own batch of prompts (weak scaling, no
@@ -56,7 +59,7 @@ def forwards_per_sample_call(S, n, mis):
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md recipe) during the timed region
+# clocks sampling (nvidia-smi queries) during the timed region
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -320,7 +323,7 @@ def roofline_pass(model, device, peaks):
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=device)
     agg = {}
     for _ in range(3):
-        flush.zero_()  # > L2 (126 MB) written between iterations
+        flush.zero_()  # > L2 (50 MB) written between iterations
         ops.PROFILE = []
         model.forward_batched([inp, un])
         torch.cuda.synchronize()
@@ -344,38 +347,30 @@ def roofline_pass(model, device, peaks):
         f = fam.setdefault(tgt, [0.0, 0.0, 0.0, 0])
         for i in range(4):
             f[i] += a[i]
-    traffic_tab = {}
-    try:
-        if (BATCH, LATENT) != (4, 64):  # the table was captured on forward batch 8 at 64x64 (configs 2 / 3)
-            raise KeyError("no traffic capture for this workload")
-        # DRAM bytes per launch per kernel family: `ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum` over one
-        # eager forward of this workload (tools/r2_profiles.sh -> tools/ncu_traffic.py)
-        traffic_tab = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-    except Exception:
-        pass
     dom = max(fam.items(), key=lambda kv: kv[1][0])
     kind, a = dom
-    traffic = traffic_tab.get(kind, {}).get("dram_bytes_per_launch")
+    traffic = None  # DRAM bytes per launch: not measured on H100 (no hardware counters available)
     if a[1] > 0:
         achieved = a[1] / a[0] / 1e12
-        peak = peaks.get("bf16_tflops_sustained") or 1400.0
+        peak = peaks.get("bf16_tflops_sustained") or 989.0
         roof = {"bound": "tensor", "kernel": kind, "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
                 "frac": achieved / peak, "traffic": traffic, "launches_per_forward": a[3] // 3,
                 "share_of_forward": a[0] / tot,
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1.4 PFLOP/s sustained"}
+                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks
+                else "fallback: H100 SXM data sheet, 989 TFLOP/s dense bf16 at 700 W"}
     else:
         achieved = a[2] / a[0] / 1e9
-        peak = peaks.get("hbm_gbs") or 6650.0
+        peak = peaks.get("hbm_gbs") or 3350.0
         roof = {"bound": "hbm", "kernel": kind, "achieved": achieved, "peak": peak, "unit": "GB/s",
                 "frac": achieved / peak, "traffic": traffic,
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6.65 TB/s"}
+                "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback: H100 SXM data sheet, 3.35 TB/s"}
     # the north-star kernel (fused gated self-attention at the 64x64 level) reported next to it
     att = agg.get("attention_d40")
     if att and att[0] > 0:
-        peak = peaks.get("bf16_tflops_sustained") or 1400.0
+        peak = peaks.get("bf16_tflops_sustained") or 989.0
         roof["attention_d40"] = {"achieved": att[1] / att[0] / 1e12, "unit": "TFLOP/s", "frac": att[1] / att[0] / 1e12 / peak,
                                  "share_of_forward": att[0] / tot,
-                                 "traffic": traffic_tab.get("attention2_kernel", {}).get("dram_bytes_per_launch")}
+                                 "traffic": None}
     n_launch = sum(a[3] for a in agg.values()) // 3
     return roof, breakdown, n_launch
 
@@ -395,6 +390,8 @@ def main():
     ap.add_argument("--dtype", default=None, choices=["fp16", "bf16"],
                     help="16-bit storage type (default: the config's own -- fp16, bf16 for config 4)")
     ap.add_argument("--no-mis-leg", action="store_true", help="skip the extra mis=0.36 leg of config 2")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the latents of the last timed step to DIR/latent.npy (float32)")
     args = ap.parse_args()
     _claim_stdout()
     cfg = CONFIGS[args.config]
@@ -481,10 +478,16 @@ def main():
         t_e2e = parallel.max_over_ranks(ev2[0].elapsed_time(ev2[1]) * 1e-3, device)
         images = BATCH * steps * world
         return dict(value=images / t_dev, e2e=images / t_e2e, ms_per_step=t_dev / steps * 1e3, h2d=h2d_bytes,
-                    d2h=result_host.numel() * 4, clocks=clk.summary(), fpc=forwards_per_sample_call(S_STEPS, N_INST, mis))
+                    d2h=result_host.numel() * 4, clocks=clk.summary(), fpc=forwards_per_sample_call(S_STEPS, N_INST, mis),
+                    out=out.float().cpu())
 
-    peak_tf = peaks.get("bf16_tflops_sustained") or 1400.0
+    peak_tf = peaks.get("bf16_tflops_sustained") or 989.0
     head = measure(args.mis, args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:
+        # the latents (B, 4, H/8, W/8) the last resident timed sample() call returned: 256 KB at config 2
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "latent.npy"), head["out"].numpy().astype(np.float32))
     # The reference's stock sampler is the Multi-instance Sampler at mis=0.36 (inference.py:59-64,176): measured
     # in the same invocation (bounded: <= 3 steps) so that the driver sees both numbers.
     mis_leg = None
@@ -500,7 +503,7 @@ def main():
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": dtype_name, "data": "synthetic",
         "config": {"workload": WORKLOAD, "mis": args.mis, "global_batch": BATCH * world, "parallelism": f"dp{world}",
                    "forwards_per_call": fpc, "forward_batch": 2 * BATCH,
-                   "l2_policy": "activations per forward (>1 GB at batch 8) exceed the 126 MB L2; roofline pass "
+                   "l2_policy": "activations per forward (>1 GB at batch 8) exceed the 50 MB L2; roofline pass "
                                 "flushes L2 (256 MB write) between iterations",
                    "cuda_graph": bool(model.use_cuda_graph), "weights": "seeded random (no checkpoint offline)",
                    "weight_broadcast_bytes": sent, "weight_broadcast_ms": bcast_ms,

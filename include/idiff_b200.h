@@ -1,5 +1,5 @@
 /*
- * idiff_b200.h -- C ABI of libidiff_b200.so: the sm_100a (B200) kernels behind the
+ * idiff_b200.h -- C ABI of libidiff_b200.so: the sm_90a (H100) kernels behind the
  * InstanceDiffusion sampling hot path.
  *
  * The reference (frank-xwang/InstanceDiffusion) is pure Python/PyTorch and has no FFI; its
@@ -39,8 +39,8 @@ int idiff_version(void);
 int idiff_storage_dtype(void);
 
 /* ---------------------------------------------------------------------------------------------
- * idiff_gemm: out = epilogue(A . W^T) on tcgen05 tensor cores (TMA-staged 128B-swizzled tiles,
- * fp32 accumulation in TMEM).  Replaces every nn.Linear / 1x1 conv / 3x3 conv of the path:
+ * idiff_gemm: out = epilogue(A . W^T) on wgmma tensor cores (TMA-staged 128B-swizzled tiles,
+ * fp32 accumulation in registers).  Replaces every nn.Linear / 1x1 conv / 3x3 conv of the path:
  *   attention.py:41 (GEGLU proj), :62 (FF out), :121-125,175-179 (to_q/k/v/to_out), :297 (fuser
  *   linear), :354,363 (proj_in/proj_out 1x1); openaimodel.py:186,213 (ResBlock conv3x3), :109
  *   (Upsample conv), :134 (Downsample conv), :205 (emb_layers), :361-363 (time_embed), :464 (out);
@@ -102,13 +102,14 @@ int idiff_row_stats(const void* x, void* stats, int rows, int channels, void* st
  * GEMM runs data-parallel. */
 long idiff_gemm_workspace_bytes(void);
 int idiff_set_gemm_workspace(void* ptr, long bytes);
-/* Profiling hook: device buffer of 16 x uint64 per CTA (>= 148*16) receiving %globaltimer stamps of
- * each GEMM CTA's phases (tools/trace_gemm.py names them); NULL (default) disables it. */
+/* Profiling hook: device buffer of 16 x uint64 per CTA (>= SM count * 16) receiving %globaltimer stamps of
+ * each GEMM CTA's entry (slot 0) and exit (slot 7) and its SM clock at entry / exit (slots 12 / 13); NULL (default)
+ * disables it. */
 int idiff_set_gemm_trace(void* ptr);
 
 /* ---------------------------------------------------------------------------------------------
  * idiff_attention: softmax(Q K^T * scale) V per (batch, head), flash-style online softmax with
- * S/O accumulators in TMEM.  Keys/values come from up to two segments: segment 0 = the visual
+ * S/O accumulators in registers.  Keys/values come from up to two segments: segment 0 = the visual
  * tokens (or the 77 text tokens), segment 1 = the 184 UniFusion object tokens of
  * GatedSelfAttentionDense (attention.py:304-309) -- queries exist only for the visual rows, which
  * is exactly the slice the reference keeps (:308).  Replaces F.scaled_dot_product_attention at

@@ -1,5 +1,5 @@
-"""instancediffusion_b200 -- B200-native (sm_100a) kernels + drop-in host mirror for the
-InstanceDiffusion sampling hot path (SURVEY.md section 8).  See DESIGN.md."""
+"""instancediffusion_b200 -- H100-native (sm_90a) kernels + drop-in host mirror for the
+InstanceDiffusion sampling hot path (SURVEY.md section 8)."""
 
 __version__ = "0.1.0"
 

@@ -115,7 +115,7 @@ def load(kind: str | None = None) -> C.CDLL:
     path = LIB_PATHS[kind]
     if not os.path.exists(path):
         raise IdiffError(
-            f"{path} not found: the sm_100a CUDA library is required (no fallback). "
+            f"{path} not found: the sm_90a CUDA library is required (no fallback). "
             "Build it with `python -m instancediffusion_b200.build` or __graft_entry__.build()."
         )
     lib = C.CDLL(path)

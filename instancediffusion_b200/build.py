@@ -1,4 +1,4 @@
-"""Build libidiff_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libidiff_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 No torch / pybind dependency: plain `nvcc -shared`.  The .so lands next to the sources
 (instancediffusion_b200/csrc/libidiff_b200.so) so it travels with the repo snapshot.
@@ -14,11 +14,11 @@ import sys
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 LIB = os.path.join(CSRC, "libidiff_b200.so")
 LIB_BF16 = os.path.join(CSRC, "libidiff_b200_bf16.so")  # same sources, -DIDIFF_STORAGE_BF16=1 (include/idiff_b200.h)
-SOURCES = ["host.cu", "gemm2.cu", "attention.cu", "attention2.cu", "norm.cu", "scaleu.cu", "elementwise.cu", "convnext.cu", "vae.cu", "clip.cu"]
-HEADERS = ["common.cuh", "host.cuh", os.path.join("..", "..", "include", "idiff_b200.h")]
+SOURCES = ["host.cu", "gemm2.cu", "attention.cu", "norm.cu", "scaleu.cu", "elementwise.cu", "convnext.cu", "vae.cu", "clip.cu"]
+HEADERS = ["common.cuh", "host.cuh", "wgmma.cuh", os.path.join("..", "..", "include", "idiff_b200.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -71,7 +71,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if failed:
         raise RuntimeError("nvcc compilation failed")
     for lib, lobjs in objs.items():
-        link = [nvcc, "-shared", "-o", lib, *lobjs, "-gencode", "arch=compute_100a,code=sm_100a"]
+        link = [nvcc, "-shared", "-o", lib, *lobjs, "-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n" + r.stdout)

@@ -2,7 +2,7 @@
 // GEMM.  Reference: ldm/modules/diffusionmodules/convnext.py:15-123 and
 // text_grounding_net.py:226-231, 277-287.  The encoder runs once per sample (its input never changes
 // across denoising steps), so these are plain coalesced HBM kernels; the pointwise convolutions, the
-// 4x4 / 2x2 patchify convolutions and the MLP are tcgen05 GEMMs (gemm2.cu, GELU epilogue flag).
+// 4x4 / 2x2 patchify convolutions and the MLP are wgmma GEMMs (gemm2.cu, GELU epilogue flag).
 //
 //   segs (B,30,S,S) fp32 --nearest resize to 512, conv3x3 30->3-->  NHWC fp16 (B,512,512,3)   [segs_inconv]
 //   patchify p x p (stride p)  -> [B*(H/p)*(W/p), p*p*C] rows for the strided-conv GEMMs       [patchify]
@@ -194,7 +194,7 @@ __global__ void seg_tokens_kernel(const h16* __restrict__ feat, const h16* __res
 
 static int grid_for(long total, int block) {
   long g = (total + block - 1) / block;
-  if (g > 148L * 32) g = 148L * 32;
+  if (g > num_sms() * 32L) g = num_sms() * 32L;
   if (g < 1) g = 1;
   return (int)g;
 }

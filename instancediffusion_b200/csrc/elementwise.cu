@@ -202,7 +202,7 @@ __global__ void silu_f16_kernel(const h16* __restrict__ x, h16* __restrict__ y, 
 
 static inline int grid_for(long total, int threads) {
   long g = (total + threads - 1) / threads;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > num_sms() * 16) g = num_sms() * 16;
   if (g < 1) g = 1;
   return (int)g;
 }

@@ -85,6 +85,17 @@ bool pdl_enabled() {
   return on;
 }
 
+int num_sms() {
+  static const int n = []() {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        v <= 0)
+      v = 132;  // H100 SXM
+    return v;
+  }();
+  return n;
+}
+
 }  // namespace idiff
 
 extern "C" const char* idiff_last_error(void) { return idiff::g_err; }

@@ -38,11 +38,13 @@ int encode_tmap_f16_sw(CUtensorMap* map, const void* base, int rank, const uint6
 // Launch with programmatic stream serialization ("programmatic dependent launch"): the kernel may
 // become resident while its predecessor in the stream is still running; every kernel of this library
 // calls pdl_wait() (common.cuh) before it touches global memory, so only launch latency and prologues
-// (barrier init, TMEM allocation, descriptor prefetch) overlap.  About 500 dependent launches make one
+// (barrier init, descriptor prefetch) overlap.  About 500 dependent launches make one
 // UNet forward.  Opt-in with IDIFF_PDL=1: measured neutral inside the CUDA graph (the big kernels fill
 // the register file, so a successor cannot become resident before they exit); plain stream order is
 // the default.
 bool pdl_enabled();
+// multiprocessor count of the current device (queried once; grid sizes of the bandwidth-bound kernels)
+int num_sms();
 template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
                        Args&&... args) {

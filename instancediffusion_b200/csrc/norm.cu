@@ -29,9 +29,7 @@ IDIFF_DEVICE void unpack8(const uint4& v, float (&f)[8]) {
 }
 
 // grid (chunks, B), block k*CV.  partial: [B][groups][GN_MAX_CHUNKS] (sum, sumsq) pairs, chunk fastest, so that the
-// apply pass reduces a group's chunks with coalesced loads and a butterfly.  (Measured, round 2: 512-thread CTAs with
-// eight loads in flight per thread and half as many chunks were SLOWER -- 4096x320: 42 vs 38 us for the pair -- the
-// pass is bound by CTA count / tail, not by loads in flight; profiles/r2_ncu_gn_stats_kernel.summary.csv.)
+// apply pass reduces a group's chunks with coalesced loads and a butterfly.
 __global__ void __launch_bounds__(512)
 gn_stats_kernel(const uint4* __restrict__ x, float* __restrict__ partial, int hw, int C, int groups,
                 int pix_per_block, int k) {
@@ -539,7 +537,7 @@ static void gn_geometry(int batch, int hw, int channels, int* k, int* ppb, int* 
   if (kk < 1) kk = 1;
   if (kk > hw) kk = hw;
   // aim at >= ~4 CTAs per SM over the whole launch, at most GN_MAX_CHUNKS chunks per sample
-  int want = (148 * 4 + batch - 1) / batch;
+  int want = (idiff::num_sms() * 4 + batch - 1) / batch;
   if (want > idiff::GN_MAX_CHUNKS) want = idiff::GN_MAX_CHUNKS;
   if (want < 1) want = 1;
   int p = (hw + want - 1) / want;
@@ -574,9 +572,9 @@ static bool gn_fused_geometry(int batch, int hw, int channels, int groups, int* 
   *CL = cl;
   *k = kk;
   *smem = (size_t)(hw / cl) * cs * 2 + (size_t)kk * cs * 2 * sizeof(float);
-  // Measured (profiles/README.md, NEXT.md): with these 100-190 KB tiles the single pass wins only while
-  // the whole launch is resident at once; beyond one wave the two-kernel path is faster.
-  if ((long)batch * (channels / cs) * cl > 148) return false;
+  // With these 100-190 KB tiles the single pass is only used while the whole launch is resident at once
+  // (one wave); beyond that the two-kernel path runs.
+  if ((long)batch * (channels / cs) * cl > idiff::num_sms()) return false;
   return *smem <= 200 * 1024;
 }
 
@@ -590,8 +588,7 @@ extern "C" int idiff_groupnorm(const void* x, void* y, const float* gamma, const
   IDIFF_REQUIRE(channels % 8 == 0 && channels <= 4096, "idiff_groupnorm: C=%d must be a multiple of 8, <= 4096", channels);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   {
-    // Single-pass cluster kernel wherever the launch fits one wave (gn_fused_geometry): measured 42 -> 31 us at
-    // 4096x320, 36 -> 21 at 1024x640, 26 -> 16 at 256x1280, 22 -> 12 at 64x1280 (batch 8; profiles/README.md);
+    // Single-pass cluster kernel wherever the launch fits one wave (gn_fused_geometry);
     // IDIFF_GN_FUSED=0 forces the two-kernel path (read per call so tests can cover both).
     const char* fe = getenv("IDIFF_GN_FUSED");
     const bool fused_on = !(fe && fe[0] == '0');

@@ -184,7 +184,7 @@ static void su_geometry(int batch, int hw, int cv, int max_chunks, int* k, int* 
   int kk = 256 / cv;  // (512-thread CTAs with half as many chunks measured slower, like the GroupNorm passes)
   if (kk < 1) kk = 1;
   if (kk > hw) kk = hw;
-  int want = (148 * 3 + batch - 1) / batch;
+  int want = (num_sms() * 3 + batch - 1) / batch;
   if (want > max_chunks) want = max_chunks;
   if (want < 1) want = 1;
   int p = (hw + want - 1) / want;

@@ -3,7 +3,7 @@
 //   * latent prologue: z / scale_factor, post_quant_conv (1x1, 4 -> 4), fp32 NCHW -> fp16 NHWC padded to
 //     the 64-channel granularity of the conv3x3 kernel's A operand;
 //   * row softmax of the single-head mid-block attention (AttnBlock, model.py:150-202): the scores of one
-//     image are a [HW, HW] GEMM output (head_dim 512 does not fit the flash kernels' TMEM budget and the
+//     image are a [HW, HW] GEMM output (head_dim 512 does not fit the flash kernels' register tiles and the
 //     block runs once per image), normalised in place.
 #include "../../include/idiff_b200.h"
 #include "common.cuh"
@@ -110,7 +110,7 @@ extern "C" int idiff_vae_latent_in(const float* z, const float* w, const float* 
   IDIFF_REQUIRE(z && w && bias && out, "idiff_vae_latent_in: null pointer argument");
   IDIFF_REQUIRE(channels >= 1 && channels <= 8, "idiff_vae_latent_in: 1..8 latent channels supported (got %d)", channels);
   const long total = (long)batch * hw;
-  const int blocks = (int)((total + 255) / 256 < 148 * 8 ? (total + 255) / 256 : 148 * 8);
+  const int blocks = (int)((total + 255) / 256 < num_sms() * 8 ? (total + 255) / 256 : num_sms() * 8);
   IDIFF_CHECK_CUDA(launch_pdl(vae_latent_in_kernel, dim3(blocks), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), z, w,
                               bias, inv_scale, reinterpret_cast<uint4*>(out), batch, channels, hw));
   IDIFF_CHECK_CUDA(cudaGetLastError());

@@ -48,7 +48,7 @@ _FIRST_STAGE = {
     "ldm.models.autoencoder": "instancediffusion_b200.ldm.models.autoencoder",
     "ldm.modules.diffusionmodules.model": "instancediffusion_b200.ldm.modules.diffusionmodules.model",
 }
-# opt-in (install(text_encoder=True)): the CLIP text tower of FrozenCLIPEmbedder on the B200 kernels; the other
+# opt-in (install(text_encoder=True)): the CLIP text tower of FrozenCLIPEmbedder on the H100 kernels; the other
 # encoder classes of that file (BERT, FrozenCLIPTextEmbedder, ...) are fetched lazily from the reference's own file
 _TEXT_ENCODER = {
     "ldm.modules.encoders.modules": "instancediffusion_b200.ldm.modules.encoders.modules",

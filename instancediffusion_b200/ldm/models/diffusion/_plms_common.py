@@ -1,6 +1,6 @@
 """Shared machinery of the two PLMS samplers (plms.py / plms_instance.py of the reference).
 
-B200-first restructuring of `p_sample_plms` (plms.py:117-167 == plms_instance.py:162-212):
+GPU-first restructuring of `p_sample_plms` (plms.py:117-167 == plms_instance.py:162-212):
   * the conditional and unconditional UNet evaluations -- and, during the Multi-instance phase,
     those of all n+1 trajectories -- are ONE batched forward (`UNetModel.forward_batched`);
   * classifier-free guidance, the Adams-Bashforth combination and the x_{t-1} update are one fused

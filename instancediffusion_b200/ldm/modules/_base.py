@@ -58,7 +58,7 @@ class PackedModule(nn.Module):
 def dev_of(p: torch.Tensor) -> torch.device:
     if not p.is_cuda:
         raise _lib.IdiffError(
-            "instancediffusion_b200 modules run only on a CUDA device (sm_100a); there is no CPU path. "
+            "instancediffusion_b200 modules run only on a CUDA device (sm_90a); there is no CPU path. "
             "Move the module with .cuda() first.")
     return p.device
 

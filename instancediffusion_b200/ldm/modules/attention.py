@@ -1,6 +1,6 @@
 """Transformer operators of the UNet, same class names / constructor and forward signatures /
 state_dict keys as the reference's ldm/modules/attention.py, with the arithmetic in
-libidiff_b200.so (tcgen05 GEMM + flash attention + LayerNorm/GroupNorm kernels).
+libidiff_b200.so (wgmma GEMM + flash attention + LayerNorm/GroupNorm kernels).
 
 Internal convention: token-major fp16 activations `[B*N, C]` (== NHWC), carried between the
 `_fwd` methods without any NCHW<->(B,HW,C) rearrange (attention.py:369,376 disappear).

@@ -3,9 +3,9 @@
 load strict).  It only runs when a sample carries non-zero `segs` (mask conditioning,
 text_grounding_net.py:226-231), once per sample after hoisting.
 
-B200 mapping (activations NHWC fp16 == token-major rows):
+H100 mapping (activations NHWC fp16 == token-major rows):
   * stem Conv2d(3, 96, 4, stride 4) and the three Conv2d(C, 2C, 2, stride 2) downsamplers are
-    kernel == stride convolutions: one coalesced patch gather (idiff_patchify) + a tcgen05 GEMM;
+    kernel == stride convolutions: one coalesced patch gather (idiff_patchify) + a wgmma GEMM;
   * Block = depthwise 7x7 (idiff_dwconv7x7) -> LayerNorm over channels (idiff_layernorm; with NHWC rows the
     reference's permutes vanish) -> pwconv1 GEMM with the exact-erf GELU fused in the epilogue ->
     pwconv2 GEMM whose epilogue adds the block input; the layer-scale `gamma` is folded into pwconv2's

@@ -3,10 +3,10 @@ ldm/modules/diffusionmodules/openaimodel.py (same class names, constructor kwarg
 signatures, attributes and the 1199 state_dict keys of SURVEY.md appendix B), executing on
 libidiff_b200.so.
 
-B200-first restructuring of `UNetModel.forward_single_input` (openaimodel.py:482-563); each item is
+GPU-first restructuring of `UNetModel.forward_single_input` (openaimodel.py:482-563); each item is
 exact in real arithmetic (SURVEY.md section 7):
   * activations stay fp16 NHWC == token-major from the first conv to the last; every conv / linear
-    is one tcgen05 GEMM whose epilogue carries bias, time-embedding add, residual, gate, GEGLU;
+    is one wgmma GEMM whose epilogue carries bias, time-embedding add, residual, gate, GEGLU;
   * step-invariant work is hoisted and cached: UniFusion object tokens and their per-fuser K/V,
     the text K/V of the 16 cross-attentions (one batched GEMM), and per step one batched GEMM for
     the 22 ResBlock time-embedding projections;
@@ -586,7 +586,7 @@ class UNetModel(PackedModule):
         """Concatenate independent forwards (cond / uncond / MIS trajectories) along the batch.  The step-invariant
         parts -- text K/V, per-fuser object K/V, mask words -- are concatenated once per combination of inputs and
         reused on every later step (the same tensor objects come back, which lets `_CoreGraph.replay` skip its copies
-        as well): 17-19 torch.cat launches and as many copies per forward otherwise (profiles/README.md round 2)."""
+        as well): 17-19 torch.cat launches and as many copies per forward otherwise."""
         xs, ts, ctxs, okv_lists, masks, bs = [], [], [], [], [], []
         active = self._fusers_active()
         n_obj = 0

@@ -4,9 +4,9 @@
 MLPs, plus 64 mask tokens -> a fifth MLP; padded / dropped slots take learned null features.
 Output (B, 30*4 + 64 = 184, 768) and `drop_box_mask`.
 
-B200 mapping: one coalesced kernel per modality builds the MLP input matrix (Fourier embedding,
+H100 mapping: one coalesced kernel per modality builds the MLP input matrix (Fourier embedding,
 null substitution and the text concat fused, idiff_fourier_embed); the MLPs are weight-streaming
-tcgen05 GEMMs with SiLU epilogues.  The result depends only on the sample's conditioning, so the
+wgmma GEMMs with SiLU epilogues.  The result depends only on the sample's conditioning, so the
 UNet calls this once per sample, not once per forward (text_grounding_net.py is re-run on every
 forward in the reference, openaimodel.py:494).
 """

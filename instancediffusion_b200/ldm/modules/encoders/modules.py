@@ -1,4 +1,4 @@
-"""CLIP text encoder on the B200 kernels -- drop-in for the text side of ldm/modules/encoders/modules.py:144-172
+"""CLIP text encoder on the H100 kernels -- drop-in for the text side of ldm/modules/encoders/modules.py:144-172
 (`FrozenCLIPEmbedder`: prompt -> (B, 77, 768) context, optionally the pooled feature) and for the phrase features
 of utils/model.py:130-152 (`get_clip_feature`: `outputs.text_model_output.pooler_output` of the same text tower).
 
@@ -149,7 +149,7 @@ class CLIPTextModel(PackedModule):
 
 
 class FrozenCLIPEmbedder(AbstractEncoder):
-    """ldm/modules/encoders/modules.py:144-172 with the text tower on the B200 kernels.  `tokenizer`: any callable with
+    """ldm/modules/encoders/modules.py:144-172 with the text tower on the H100 kernels.  `tokenizer`: any callable with
     the CLIPTokenizer call signature; by default transformers.CLIPTokenizer.from_pretrained(version) is tried and, if
     its files are not available (offline), left None -- `forward` then accepts a LongTensor of token ids."""
 

@@ -1,4 +1,4 @@
-"""`-m gpu` tests of the CLIP text encoder on the B200 kernels (host prep, SURVEY.md section 8f-3): the two small kernels
+"""`-m gpu` tests of the CLIP text encoder on the H100 kernels (host prep, SURVEY.md section 8f-3): the two small kernels
 against torch, the whole text tower against the golden produced by transformers' CLIPTextModel (the third-party model
 the reference calls at ldm/modules/encoders/modules.py:147-165 and utils/model.py:146-151), the FrozenCLIPEmbedder /
 get_clip_feature surface, and the bf16 build."""
@@ -15,7 +15,7 @@ import cases  # noqa: E402
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(HERE, "golden")
 
-# measured on B200: text tower rel-L2 1.2e-3 (fp16 storage), 9.6e-3 (bf16); bounds <= 2x measured
+# bounds: about 2x the measured text-tower errors
 CLIP_TOL = 2.4e-3
 
 

@@ -159,7 +159,7 @@ def test_unet_eps_matches_reference_golden(cuda_device, unet):
     objs, _ = unet.position_net(gi["boxes"], gi["masks"], gi["positive_embeddings"], gi["scribbles"], gi["polygons"],
                                 gi["segs"], gi["points"])
     _report(objs, gold["objs"], "unet/objs", 1.1e-3, 1.2e-3)
-    # one full denoise forward: ~200 fp16 layers deep.  Measured 2.0e-3 relative L2 (DESIGN.md section 7);
+    # one full denoise forward: ~200 fp16 layers deep.  Bound about 2x the measured relative L2;
     # the bound is 2x that.  (The reference itself under autocast(fp16) deviates as much:
     # tests/test_parity_r2_gpu.py::test_fp16_envelope_eps_and_latents.)
     for graph in (False, True):

@@ -2,7 +2,7 @@
 SURVEY.md section 8f-1) against the reference's own fp32 output (tests/golden/vae.pt, oracle/make_golden.py
 --only vae), plus the kernels that exist only for it.  The reference decodes in fp32 (inference.py:96 is
 outside the autocast region); here activations are fp16 with fp32 accumulation / statistics, so the bound is
-an fp16 one: relative L2 of the image, stated per test at <= 2x the value measured on the B200."""
+an fp16 one: relative L2 of the image, stated per test at about 2x the measured value."""
 import os
 import sys
 
