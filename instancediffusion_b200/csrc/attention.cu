@@ -1,12 +1,13 @@
 // Flash-style attention on wgmma for sm_90a: O = softmax(Q K^T * scale) V per (batch, head).
 //
 // One CTA owns a 128-query tile of one (batch, head): warpgroup 0 is the TMA producer (Q once, then
-// K / V tiles of 64 keys through a ring), warpgroups 1 and 2 each own 64 query rows.  Per key block a
-// consumer warpgroup computes S = Q K^T with wgmma (Q and K from 128B-swizzled shared memory) into
-// registers, runs the online softmax on the fragments (a row lives in the four threads of a quad),
-// and feeds P straight from registers as the A operand of O += P V; V is consumed as an MN-major B
-// operand from its token-major tile, so no transposed copy of V is ever made.  O stays in registers
-// and is normalised and stored at the end.
+// K / V tiles of 128 keys at d = 40, 64 keys otherwise, through a ring), warpgroups 1 and 2 each own
+// 64 query rows.  Per key block a consumer warpgroup computes S = Q K^T with wgmma (Q and K from
+// 128B-swizzled shared memory) into registers, runs the online softmax on the fragments (a row lives
+// in the four threads of a quad), and feeds P straight from registers as the A operand of O += P V
+// at N = d; V is consumed as an MN-major B operand from its token-major tile, so no transposed copy
+// of V is ever made.  The PV product of block j - 1 runs on the tensor cores during the softmax of
+// block j.  O stays in registers and is normalised and stored at the end.
 // Keys/values are read from up to two segments (visual tokens, then the 184 UniFusion object
 // tokens of GatedSelfAttentionDense) -- the concatenation of attention.py:306 never exists.
 // The optional instance-isolation mask (attention.py:187-255) is applied to the scores: query i may
@@ -23,7 +24,6 @@ namespace idiff {
 
 constexpr int ATT_THREADS = 384;
 constexpr int BQ = 128;
-constexpr int BKV = 64;
 
 struct AttnKParams {
   int heads, nq, n0, n1, kv1_broadcast;
@@ -38,7 +38,9 @@ template <int D>
 struct AttnCfg {
   static constexpr int ND = (D + 63) / 64;           // 64-wide d chunks (one TMA box each)
   static constexpr int KSTEPS = (D + 15) / 16;       // wgmma k-steps of QK^T (zero padded)
-  static constexpr int DV = ND * 64;                 // wgmma N of the PV product
+  // keys per block: at d = 40 a 64-key block is too little work to amortise a block's fixed cost (ring
+  // waits, wgmma issue and latency, row-max shuffles, O rescale); at d >= 80 S + P + O must fit in registers
+  static constexpr int BKV = (D <= 64) ? 128 : 64;
   static constexpr int STAGES = (D <= 64) ? 4 : 3;
   static constexpr int Q_BYTES = ND * BQ * 128;
   static constexpr int KV_TILE_BYTES = ND * BKV * 128;  // one of K or V
@@ -51,7 +53,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
                  const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
                  const __grid_constant__ CUtensorMap tmV1, const AttnKParams p) {
   using Cfg = AttnCfg<D>;
-  constexpr int ND = Cfg::ND, STAGES = Cfg::STAGES, DV = Cfg::DV;
+  constexpr int ND = Cfg::ND, STAGES = Cfg::STAGES, BKV = Cfg::BKV;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -119,12 +121,18 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
     // ===================== consumers: S = Q K^T, online softmax, O += P V =====================
+    // Per key block j a consumer issues S_j = Q K_j^T and O += P_{j-1} V_{j-1} back to back, runs the
+    // softmax of S_j while the PV product is still on the tensor cores, then waits for it and rescales O.
+    // The two consumer warpgroups also take turns issuing (named barrier 1 + cw grants warpgroup cw its
+    // turn), so one warpgroup's softmax runs under the other's wgmmas.
     const int cw = (warp >> 2) - 1;  // rows [64 cw, 64 cw + 64) of the query tile
+    const uint32_t my_turn = 1 + cw, their_turn = 2 - cw;
     const int t4 = lane & 3;
     const int rl0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);  // tile rows of this thread: rl0, rl0 + 8
     const float c = p.scale_log2e;
     // descriptors: Q / K K-major (rows of 128 B, 8-row atoms 1024 B apart); V MN-major (64-wide d atoms
-    // BKV * 128 B apart, 8-key groups 1024 B apart)
+    // BKV * 128 B apart, 8-key groups 1024 B apart).  The PV product runs at N = D: it reads the first D
+    // columns of the zero-padded 64-wide V boxes.
     const uint64_t dq = make_wgmma_desc(smem_u32(sQ) + cw * 64 * 128, 16, 1024);
     const uint64_t dk = make_wgmma_desc(smem_u32(sK), 16, 1024);
     const uint64_t dv = make_wgmma_desc(smem_u32(sV), BKV * 128, 1024);
@@ -137,98 +145,175 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         qword[hh] = qr < p.nq ? __ldg(p.mask_q + (long)b * p.nq + qr) : 0xffffffffu;
       }
     }
-    float o[DV / 2];
+    float o[D / 2];
 #pragma unroll
-    for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
     float m_run[2] = {-INFINITY, -INFINITY};
     float l_part[2] = {0.f, 0.f};  // this thread's share of the row sums (quad-reduced at the end)
+    float sc[BKV / 2];
+    float alpha[2];
 
-    mbar_wait(q_full, 0);
-    uint32_t s = 0, ph = 0;
-    for (int j = 0; j < T; ++j) {
-      const bool seg1 = j >= T0;
-      const int key0 = seg1 ? (j - T0) * BKV : j * BKV;  // first key of the block within its segment
-      const int nv = min(BKV, (seg1 ? p.n1 : p.n0) - key0);
-      float sc[BKV / 2];
-      mbar_wait(&k_full[s], ph);
-      wgmma_fence();
+    auto issue_qk = [&](uint32_t st) {
 #pragma unroll
       for (int kk = 0; kk < Cfg::KSTEPS; ++kk)
         Wgmma<BKV>::ss(sc, dq + (((kk >> 2) * BQ * 128 + (kk & 3) * 32) >> 4),
-                       dk + ((s * Cfg::KV_TILE_BYTES + (kk >> 2) * BKV * 128 + (kk & 3) * 32) >> 4), kk > 0 ? 1u : 0u);
+                       dk + ((st * Cfg::KV_TILE_BYTES + (kk >> 2) * BKV * 128 + (kk & 3) * 32) >> 4), kk > 0 ? 1u : 0u);
       wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(sc);
-
-      // keys past the segment end, and (MASKED) keys this row may not see, score -inf
+    };
+    auto issue_pv = [&](const uint32_t (&pa)[BKV / 16][4], uint32_t st) {
 #pragma unroll
-      for (int jj = 0; jj < BKV / 8; ++jj) {
+      for (int kk = 0; kk < BKV / 16; ++kk)
+        Wgmma<D>::rs(o, pa[kk], dv + ((st * Cfg::KV_TILE_BYTES + kk * 16 * 128) >> 4), 1u);
+      wgmma_commit();
+    };
+    // online softmax of the scores of key block j (rows rl0, rl0 + 8; a row's BKV scores are spread over
+    // the quad): sc becomes P = 2^(s*c - m*c) in place, alpha the factor O has to be rescaled by
+    auto softmax = [&](int j) {
+      const bool seg1 = j >= T0;
+      const int key0 = seg1 ? (j - T0) * BKV : j * BKV;  // first key of the block within its segment
+      const int nv = min(BKV, (seg1 ? p.n1 : p.n0) - key0);
+      // (MASKED) keys this row may not see, and keys past the segment end (its last block only), score -inf
+      if (MASKED) {
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int kc = 8 * jj + 2 * t4 + e;  // key column of the block
-          if (kc >= nv) {
-            sc[4 * jj + e] = -INFINITY;
-            sc[4 * jj + 2 + e] = -INFINITY;
-          } else if (MASKED) {
-            const uint32_t kw = __ldg(p.mask_k + (long)b * (p.n0 + p.n1) + (seg1 ? p.n0 : 0) + key0 + kc);
+        for (int jj = 0; jj < BKV / 8; ++jj) {
 #pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-              const bool self = !seg1 && key0 + kc == q0 + rl0 + 8 * hh;
-              if ((kw & qword[hh]) == 0u && !self) sc[4 * jj + 2 * hh + e] = -INFINITY;
+          for (int e = 0; e < 2; ++e) {
+            const int kc = 8 * jj + 2 * t4 + e;  // key column of the block
+            if (kc < nv) {
+              const uint32_t kw = __ldg(p.mask_k + (long)b * (p.n0 + p.n1) + (seg1 ? p.n0 : 0) + key0 + kc);
+#pragma unroll
+              for (int hh = 0; hh < 2; ++hh) {
+                const bool self = !seg1 && key0 + kc == q0 + rl0 + 8 * hh;
+                if ((kw & qword[hh]) == 0u && !self) sc[4 * jj + 2 * hh + e] = -INFINITY;
+              }
             }
           }
         }
       }
-      // online softmax per row (rows rl0, rl0 + 8; a row's 64 scores are spread over the quad)
+      if (nv < BKV) {
+#pragma unroll
+        for (int jj = 0; jj < BKV / 8; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            if (8 * jj + 2 * t4 + e >= nv) {
+              sc[4 * jj + e] = -INFINITY;
+              sc[4 * jj + 2 + e] = -INFINITY;
+            }
+          }
+        }
+      }
       float mc[2];
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        float mx = -INFINITY;
+        // pairwise tree (a max is exact in any order): a log-depth dependency chain instead of a serial one
+        float m8[BKV / 8];
 #pragma unroll
-        for (int jj = 0; jj < BKV / 8; ++jj) mx = fmaxf(mx, fmaxf(sc[4 * jj + 2 * hh], sc[4 * jj + 2 * hh + 1]));
+        for (int jj = 0; jj < BKV / 8; ++jj) m8[jj] = fmaxf(sc[4 * jj + 2 * hh], sc[4 * jj + 2 * hh + 1]);
+        static_assert(BKV == 64 || BKV == 128, "row-max tree depth");
+#pragma unroll
+        for (int jj = 0; jj < BKV / 16; ++jj) m8[jj] = fmaxf(m8[jj], m8[jj + BKV / 16]);
+#pragma unroll
+        for (int jj = 0; jj < BKV / 32; ++jj) m8[jj] = fmaxf(m8[jj], m8[jj + BKV / 32]);
+#pragma unroll
+        for (int jj = 0; jj < BKV / 64; ++jj) m8[jj] = fmaxf(m8[jj], m8[jj + BKV / 64]);
+        if (BKV == 128) m8[0] = fmaxf(m8[0], m8[1]);
+        float mx = m8[0];
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
         const float m_new = fmaxf(m_run[hh], mx);
         // a row that has seen no live key yet keeps 0 as its reference: P = 0 instead of NaN
         const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-        const float alpha = exp2_approx((m_run[hh] - m_use) * c);  // m_run = -inf -> 0
+        alpha[hh] = exp2_approx((m_run[hh] - m_use) * c);  // m_run = -inf -> 0
         m_run[hh] = m_new;
         mc[hh] = m_use * c;
-        l_part[hh] *= alpha;
-#pragma unroll
-        for (int jj = 0; jj < DV / 8; ++jj) {
-          o[4 * jj + 2 * hh] *= alpha;
-          o[4 * jj + 2 * hh + 1] *= alpha;
-        }
+        l_part[hh] *= alpha[hh];
       }
-      // P = 2^(s*c - m*c) as 16-bit A fragments of the four 16-key k-steps
-      uint32_t pa[BKV / 16][4];
 #pragma unroll
-      for (int kk = 0; kk < BKV / 16; ++kk) {
+      for (int jj = 0; jj < BKV / 8; ++jj) {
 #pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          // register r of the A fragment = accumulator group 2kk + (r >> 1), row half (r & 1)
-          const int jj = 2 * kk + (r >> 1), hh = r & 1;
-          const float p0 = exp2_approx(fmaf(sc[4 * jj + 2 * hh], c, -mc[hh]));
-          const float p1 = exp2_approx(fmaf(sc[4 * jj + 2 * hh + 1], c, -mc[hh]));
+        for (int hh = 0; hh < 2; ++hh) {
+          float& p0 = sc[4 * jj + 2 * hh];
+          float& p1 = sc[4 * jj + 2 * hh + 1];
+          p0 = exp2_approx(fmaf(p0, c, -mc[hh]));
+          p1 = exp2_approx(fmaf(p1, c, -mc[hh]));
           l_part[hh] += p0 + p1;
-          pa[kk][r] = pack_half2(p0, p1);
         }
       }
-      mbar_wait(&v_full[s], ph);
-      wgmma_fence();
+    };
+    // P as the 16-bit A fragments of the BKV / 16 k-steps of 16 keys: register r of k-step kk = accumulator group
+    // 2kk + (r >> 1), row half (r & 1).  Written only once the previous PV product (which reads pa) retired.
+    uint32_t pa[BKV / 16][4];
+    auto pack_p = [&]() {
 #pragma unroll
       for (int kk = 0; kk < BKV / 16; ++kk)
-        Wgmma<DV>::rs(o, pa[kk], dv + ((s * Cfg::KV_TILE_BYTES + kk * 16 * 128) >> 4), 1u);
-      wgmma_commit();
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const int jj = 2 * kk + (r >> 1), hh = r & 1;
+          pa[kk][r] = pack_half2(sc[4 * jj + 2 * hh], sc[4 * jj + 2 * hh + 1]);
+        }
+    };
+
+    // PV_{j-2} has retired: free its K/V stage, rescale O by the factor of block j - 1 and pack P_{j-1}.
+    // Called at the top of a trip, not after the softmax: the compiler must not hoist the wait into the
+    // softmax (where it would stall on the PV product the softmax is meant to hide).
+    auto retire_pv = [&](bool release, uint32_t st) {
       wgmma_wait<0>();
       wgmma_fence_regs(o);
-      if (lane == 0) mbar_arrive(&kv_empty[s]);
-      if (++s == STAGES) {
-        s = 0;
-        ph ^= 1;
+      if (release && lane == 0) mbar_arrive(&kv_empty[st]);
+      // alpha is exactly 1 where the row max did not move (most blocks once a row has seen a few):
+      // skip the multiply when that holds for every row of the warp
+      if (!__all_sync(0xffffffffu, alpha[0] == 1.f && alpha[1] == 1.f)) {
+#pragma unroll
+        for (int jj = 0; jj < D / 8; ++jj) {
+          o[4 * jj] *= alpha[0];
+          o[4 * jj + 1] *= alpha[0];
+          o[4 * jj + 2] *= alpha[1];
+          o[4 * jj + 3] *= alpha[1];
+        }
       }
+      pack_p();
+    };
+
+    mbar_wait(q_full, 0);
+    if (cw == 1) named_bar_arrive(1, 256);  // warpgroup 0 takes the first turn
+    named_bar_sync(my_turn, 256);
+    mbar_wait(&k_full[0], 0);
+    wgmma_fence();
+    issue_qk(0);
+    named_bar_arrive(their_turn, 256);
+    wgmma_wait<0>();
+    wgmma_fence_regs(sc);
+    softmax(0);
+    uint32_t s = 0, ph = 0;  // ring stage / phase of block j - 1
+    uint32_t s_prev = 0;     // ring stage of block j - 2
+    for (int j = 1; j < T; ++j) {
+      retire_pv(j >= 2, s_prev);
+      const uint32_t sn = (s + 1 == STAGES) ? 0u : s + 1, phn = (sn == 0) ? ph ^ 1u : ph;
+      named_bar_sync(my_turn, 256);
+      mbar_wait(&k_full[sn], phn);
+      wgmma_fence();
+      issue_qk(sn);
+      mbar_wait(&v_full[s], ph);
+      wgmma_fence();  // ptxas would otherwise insert this fence itself after the wait loop
+      issue_pv(pa, s);
+      named_bar_arrive(their_turn, 256);
+      wgmma_wait<1>();  // S_j has landed; PV_{j-1} may still run
+      wgmma_fence_regs(sc);
+      softmax(j);
+      s_prev = s;
+      s = sn;
+      ph = phn;
     }
+    retire_pv(T >= 2, s_prev);
+    // the last PV product; warpgroup 1's turn is the last of all, so it grants none
+    named_bar_sync(my_turn, 256);
+    mbar_wait(&v_full[s], ph);
+    wgmma_fence();
+    issue_pv(pa, s);
+    if (cw == 0) named_bar_arrive(their_turn, 256);
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    if (lane == 0) mbar_arrive(&kv_empty[s]);
 
     // epilogue: O / l -> 16-bit
 #pragma unroll
@@ -241,11 +326,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       if (qrow >= p.nq) continue;
       h16* orow = p.out + ((long)b * p.nq + qrow) * p.out_ld + h * D;
 #pragma unroll
-      for (int jj = 0; jj < DV / 8; ++jj) {
-        const int col = 8 * jj + 2 * t4;
-        if (col < D)
-          *reinterpret_cast<uint32_t*>(orow + col) = pack_half2(o[4 * jj + 2 * hh] * inv_l, o[4 * jj + 2 * hh + 1] * inv_l);
-      }
+      for (int jj = 0; jj < D / 8; ++jj)
+        *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * t4) =
+            pack_half2(o[4 * jj + 2 * hh] * inv_l, o[4 * jj + 2 * hh + 1] * inv_l);
     }
   }
 }
@@ -265,12 +348,12 @@ static int launch_attention(const idiff_attn_args* a, cudaStream_t stream) {
   using Cfg = AttnCfg<D>;
   CUtensorMap tmQ, tmK0, tmV0, tmK1, tmV1;
   if (make_head_tmap(&tmQ, a->q, D, a->heads, a->nq, a->batch, a->q_ld, BQ)) return -1;
-  if (make_head_tmap(&tmK0, a->k0, D, a->heads, a->n0, a->batch, a->k0_ld, BKV)) return -1;
-  if (make_head_tmap(&tmV0, a->v0, D, a->heads, a->n0, a->batch, a->v0_ld, BKV)) return -1;
+  if (make_head_tmap(&tmK0, a->k0, D, a->heads, a->n0, a->batch, a->k0_ld, Cfg::BKV)) return -1;
+  if (make_head_tmap(&tmV0, a->v0, D, a->heads, a->n0, a->batch, a->v0_ld, Cfg::BKV)) return -1;
   if (a->n1 > 0) {
     const int b1 = a->kv1_batch == 1 ? 1 : a->batch;
-    if (make_head_tmap(&tmK1, a->k1, D, a->heads, a->n1, b1, a->k1_ld, BKV)) return -1;
-    if (make_head_tmap(&tmV1, a->v1, D, a->heads, a->n1, b1, a->v1_ld, BKV)) return -1;
+    if (make_head_tmap(&tmK1, a->k1, D, a->heads, a->n1, b1, a->k1_ld, Cfg::BKV)) return -1;
+    if (make_head_tmap(&tmV1, a->v1, D, a->heads, a->n1, b1, a->v1_ld, Cfg::BKV)) return -1;
   } else {
     tmK1 = tmK0;
     tmV1 = tmV0;

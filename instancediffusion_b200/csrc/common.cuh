@@ -103,6 +103,15 @@ IDIFF_DEVICE void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
 }
 
+// Named barriers (ids 1..15; 0 is __syncthreads): `nthreads` counts the threads of every warp that
+// syncs or arrives, so one group can wait on a barrier that another group only arrives at.
+IDIFF_DEVICE void named_bar_sync(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(nthreads) : "memory");
+}
+IDIFF_DEVICE void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;\n" ::"r"(id), "r"(nthreads) : "memory");
+}
+
 // ----------------------------------------------------------------------------------
 // TMA tiled loads (global -> shared, completion on an mbarrier)
 // ----------------------------------------------------------------------------------
