@@ -86,6 +86,11 @@ typedef struct {
   const float* ln_colsum;
   int ln_slots_in;
   float ln_eps;
+  /* Per-batch-entry residual gate (batched forwards of requests with different fuser scales): NULL, or fp32
+     [number of batch entries] -- with a residual, out = residual + gate * gate_b[b] * (...), b = row / rows_per_batch
+     (conv: the image).  Needs residual != NULL and combines with bias and ln_stats_out only (no rowadd, SiLU /
+     GELU, ln_stats_in); NULL leaves the epilogue as above. */
+  const float* gate_b;
 } idiff_gemm_args;
 int idiff_gemm(const idiff_gemm_args* args, void* stream);
 /* number of column slots a producer GEMM with these arguments writes to ln_stats_out (depends on the

@@ -30,6 +30,7 @@ class GemmArgs(C.Structure):
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_long),
         ("ln_stats_out", C.c_void_p), ("ln_stats_in", C.c_void_p), ("ln_colsum", C.c_void_p),
         ("ln_slots_in", C.c_int), ("ln_eps", C.c_float),
+        ("gate_b", C.c_void_p),
     ]
 
 

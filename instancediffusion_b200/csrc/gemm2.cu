@@ -49,6 +49,7 @@ struct Params {
   void* out;
   int ldo, ldr, ldra, rows_per_batch, flags;
   float gate;
+  const float* gate_b;  // optional per-batch-entry factor of the residual gate (header: gate_b)
   // stream-K fixup
   float* ws;    // [G][BN/8][256 consumer threads][4] fp32 partial tiles, in accumulator-fragment order
   int* sflags;  // [G][CONSUMER_WARPS] publish flags (fixed location, self-resetting)
@@ -125,6 +126,7 @@ IDIFF_DEVICE float2 ld_pair(const h16* p) { return unpack_half2(*reinterpret_cas
 constexpr int MODE_PLAIN = 0;  // bias / row-add, optional SiLU / GELU, optional gate*x + residual, fp16 out
 constexpr int MODE_GEGLU = 1;  // (value + b) * gelu(gate + b), fp16 out with N/2 columns
 constexpr int MODE_NCHW = 2;   // fp32 (B, N, HW) output (the final conv -> eps)
+constexpr int MODE_GATED = 3;  // bias, gate * gate_b[batch entry] * x + residual, fp16 out (per-image fuser scales)
 
 template <int BN, int MODE>
 __global__ void __launch_bounds__(THREADS, 1)
@@ -236,10 +238,11 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     const int rl0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);
     constexpr bool geglu = (MODE == MODE_GEGLU);
     constexpr bool nchw = (MODE == MODE_NCHW);
+    constexpr bool gated = (MODE == MODE_GATED);
     constexpr int NJ = BN / 8;                     // 8-column groups of the accumulator
     constexpr int NJO = geglu ? NJ / 2 : NJ;       // ... that produce output columns
-    const bool do_silu = (p.flags & IDIFF_EPI_SILU) != 0;
-    const bool do_gelu = (p.flags & IDIFF_EPI_GELU) != 0;
+    const bool do_silu = !gated && (p.flags & IDIFF_EPI_SILU) != 0;
+    const bool do_gelu = !gated && (p.flags & IDIFF_EPI_GELU) != 0;
     const int n_out_total = geglu ? p.N / 2 : p.N;
     // K-major SWIZZLE_128B descriptors of stage 0; a stage / 16-deep k-step is an address offset (>> 4)
     const uint64_t da0 = make_wgmma_desc(smem_u32(sA) + cw * 64 * 128, 16, 1024);
@@ -345,7 +348,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       }
       // LayerNorm fold, consumer side: each row's mean / rstd from the producer GEMM's partial sums, added in
       // slot order (deterministic).  y = rstd * (x . W'^T - mean * colsum(W')) + (W beta + b).
-      const bool lni = p.ln_in != nullptr;
+      const bool lni = !gated && p.ln_in != nullptr;
       float ln_rstd[2] = {1.f, 1.f}, ln_nmean[2] = {0.f, 0.f};
       if (lni) {
 #pragma unroll
@@ -369,6 +372,13 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       const bool lno = p.ln_out != nullptr;
       float ln_ps[2] = {0.f, 0.f}, ln_pq[2] = {0.f, 0.f};
       const float gate = p.gate;
+      // MODE_GATED: the residual gate of each row is gate * gate_b[its batch entry]
+      float gate_r[2] = {gate, gate};
+      if (gated) {
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+          if (rok[hh]) gate_r[hh] = gate * __ldg(p.gate_b + bidx[hh]);
+      }
 #pragma unroll
       for (int j = 0; j < NJO; ++j) {
         const int c = 8 * j + 2 * t4;  // tile column of the pair (GEGLU: value column; its gate is BN/2 further on)
@@ -408,7 +418,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
             x0 *= gelu_erf_f(g0);
             x1 *= gelu_erf_f(g1);
           } else {
-            if (p.rowadd) {
+            if (!gated && p.rowadd) {
               const float2 f = ld_pair(p.rowadd + (long)bidx[hh] * p.ldra + n0 + c);
               x0 += f.x;
               x1 += f.y;
@@ -429,8 +439,9 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           } else {
             if (has_res) {
               const float2 r = ld_pair(p.residual + orow[hh] * p.ldr + oc);
-              x0 = fmaf(gate, x0, r.x);
-              x1 = fmaf(gate, x1, r.y);
+              const float g = gated ? gate_r[hh] : gate;
+              x0 = fmaf(g, x0, r.x);
+              x1 = fmaf(g, x1, r.y);
             }
             if (lno) {
               ln_ps[hh] += x0 + x1;
@@ -500,6 +511,7 @@ static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
   p.rows_per_batch = a->rows_per_batch > 0 ? a->rows_per_batch : a->M;
   p.flags = a->flags;
   p.gate = a->gate;
+  p.gate_b = a->gate_b;
   p.trace = g_trace;
   p.ln_out = reinterpret_cast<float2*>(a->ln_stats_out);
   p.ln_in = reinterpret_cast<const float2*>(a->ln_stats_in);
@@ -604,7 +616,8 @@ static int count_m_tiles(const idiff_gemm_args* a) {
   }
   return (a->M + BM - 1) / BM;
 }
-static Plan plan_gemm(const idiff_gemm_args* a, int fixed_bn) {  // fixed_bn: 0 = choose the tile width
+// fixed_bn: 0 = choose the tile width, at most max_bn
+static Plan plan_gemm(const idiff_gemm_args* a, int fixed_bn, int max_bn = 256) {
   const char* force = getenv("IDIFF_GEMM_PLAN");  // "bn,sk" overrides the model (tests, tuning); bn 0 = keep
   if (g_num_sms == 0) {
     int dev = 0;
@@ -617,6 +630,7 @@ static Plan plan_gemm(const idiff_gemm_args* a, int fixed_bn) {  // fixed_bn: 0 
   const int cands[4] = {256, 192, 160, 128};
   long min_pad = -1;
   for (int i = 0; i < 4; ++i) {
+    if (cands[i] > max_bn) continue;
     const long pad = (long)((a->N + cands[i] - 1) / cands[i]) * cands[i];
     if (min_pad < 0 || pad < min_pad) min_pad = pad;
   }
@@ -624,7 +638,7 @@ static Plan plan_gemm(const idiff_gemm_args* a, int fixed_bn) {  // fixed_bn: 0 
   double best_cost = -1;
   for (int i = 0; i < 4; ++i) {
     const int bn = cands[i];
-    if (fixed_bn && bn != fixed_bn) continue;
+    if ((fixed_bn && bn != fixed_bn) || bn > max_bn) continue;
     if (!fixed_bn && a->N <= 128 && bn != 128) continue;
     const long pad = (long)((a->N + bn - 1) / bn) * bn;
     if (!fixed_bn && pad > min_pad + min_pad / 14) continue;  // more than ~7 % wasted columns
@@ -654,7 +668,7 @@ static Plan plan_gemm(const idiff_gemm_args* a, int fixed_bn) {  // fixed_bn: 0 
   if (force) {
     int fbn = 0, fsk = 0;
     if (sscanf(force, "%d,%d", &fbn, &fsk) == 2) {
-      if (!fixed_bn && (fbn == 256 || fbn == 192 || fbn == 160 || fbn == 128)) best.bn = fbn;
+      if (!fixed_bn && fbn <= max_bn && (fbn == 256 || fbn == 192 || fbn == 160 || fbn == 128)) best.bn = fbn;
       best.sk = fsk != 0;
     }
   }
@@ -670,8 +684,25 @@ static Resolved resolve(const idiff_gemm_args* a) {
   // GEGLU: one 256-column accumulator tile = 128 value columns + their 128 gates (packing.py)
   if (a->flags & IDIFF_EPI_GEGLU) return {256, MODE_GEGLU, plan_gemm(a, 256).sk};
   if (a->flags & IDIFF_OUT_F32_NCHW) return {128, MODE_NCHW, plan_gemm(a, 128).sk};
+  // MODE_GATED stays at BN <= 192: its 256-wide instantiation spills (ptxas -v), the narrower ones do not
+  if (a->gate_b) {
+    const Plan pl = plan_gemm(a, 0, 192);
+    return {pl.bn, MODE_GATED, pl.sk};
+  }
   const Plan pl = plan_gemm(a, 0);
   return {pl.bn, MODE_PLAIN, pl.sk};
+}
+
+template <int MODE>
+static int launch_bn(const idiff_gemm_args* a, cudaStream_t stream, const Resolved& r) {
+  switch (r.bn) {
+    case 256:
+      if constexpr (MODE != MODE_GATED) return launch<256, MODE>(a, stream, r.sk);
+      return -1;  // (resolve never plans it)
+    case 192: return launch<192, MODE>(a, stream, r.sk);
+    case 160: return launch<160, MODE>(a, stream, r.sk);
+    default: return launch<128, MODE>(a, stream, r.sk);
+  }
 }
 
 // One instantiation per (tile width, epilogue mode): each kernel carries only its own mode's code.
@@ -679,12 +710,8 @@ int gemm_v2(const idiff_gemm_args* a, cudaStream_t stream) {
   const Resolved r = resolve(a);
   if (r.mode == MODE_GEGLU) return launch<256, MODE_GEGLU>(a, stream, r.sk);
   if (r.mode == MODE_NCHW) return launch<128, MODE_NCHW>(a, stream, r.sk);
-  switch (r.bn) {
-    case 256: return launch<256, MODE_PLAIN>(a, stream, r.sk);
-    case 192: return launch<192, MODE_PLAIN>(a, stream, r.sk);
-    case 160: return launch<160, MODE_PLAIN>(a, stream, r.sk);
-    default: return launch<128, MODE_PLAIN>(a, stream, r.sk);
-  }
+  if (r.mode == MODE_GATED) return launch_bn<MODE_GATED>(a, stream, r);
+  return launch_bn<MODE_PLAIN>(a, stream, r);
 }
 
 // slots of the LayerNorm partial statistics a producer GEMM with these arguments writes per row
@@ -716,6 +743,11 @@ extern "C" int idiff_gemm(const idiff_gemm_args* a, void* stream) {
     }
   } else {
     IDIFF_REQUIRE(!a->residual, "idiff_gemm: NCHW fp32 output excludes residual");
+  }
+  if (a->gate_b) {
+    IDIFF_REQUIRE(a->residual, "idiff_gemm: gate_b scales the gated residual and needs a residual");
+    IDIFF_REQUIRE(!a->rowadd && !a->ln_stats_in && !(a->flags & (IDIFF_EPI_SILU | IDIFF_EPI_GELU)),
+                  "idiff_gemm: gate_b combines with bias, residual and ln_stats_out only");
   }
   if (a->workspace) {
     IDIFF_REQUIRE((reinterpret_cast<uintptr_t>(a->workspace) & 255) == 0, "idiff_gemm: workspace must be 256B aligned");

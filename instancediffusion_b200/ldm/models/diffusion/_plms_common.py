@@ -100,30 +100,49 @@ class PLMSBase(object):
 
     def _step(self, trajs: List[Trajectory], ts, ts_next, index, uc, guidance_scale):
         """p_sample_plms for every trajectory in `trajs` (they share the step index)."""
-        a_t = float(self.ddim_alphas[index])
-        a_prev = float(np.float32(self.ddim_alphas_prev[index]))
-        s1m = float(self.ddim_sqrt_one_minus_alphas[index])
-        gs = float(guidance_scale)
         for tr in trajs:
             tr.input["timesteps"] = ts
         evals = self._eval(trajs, uc, guidance_scale)
+        pending = self._step_predict(trajs, evals, ts_next, index, guidance_scale)
+        if pending is not None:
+            evals = self._eval(trajs, uc, guidance_scale)
+        self._step_finish(trajs, evals, pending, index, guidance_scale)
+
+    def _coefs(self, index):
+        return (float(self.ddim_alphas[index]), float(np.float32(self.ddim_alphas_prev[index])),
+                float(self.ddim_sqrt_one_minus_alphas[index]))
+
+    def _step_predict(self, trajs: List[Trajectory], evals, ts_next, index, guidance_scale):
+        """First half of `_step` after the evaluation at t.  Trajectories without eps history take the pseudo
+        improved Euler predictor (plms.py:146-152): their inputs move to (x_pred, t_next) and the returned state
+        is finished by `_step_finish` with a second evaluation.  Returns None when one evaluation suffices."""
         first = [tr for tr in trajs if len(tr.old_eps) == 0]
+        if not first:
+            return None
+        assert len(first) == len(trajs), "trajectories must share their history length"
+        a_t, a_prev, s1m = self._coefs(index)
+        gs = float(guidance_scale)
+        x0s, e_ts = [], []
+        for tr, (e_c, e_u) in zip(trajs, evals):
+            x = tr.input["x"].float().contiguous()
+            x0s.append(x)
+            e_t = torch.empty_like(x)
+            x_pred = torch.empty_like(x)
+            ops.plms_update(x, e_c, e_u, gs, [], [1.0], a_t, a_prev, s1m, e_t, x_pred)
+            e_ts.append(e_t)
+            tr.input["x"] = x_pred
+            tr.input["timesteps"] = ts_next
+        return x0s, e_ts
+
+    def _step_finish(self, trajs: List[Trajectory], evals, pending, index, guidance_scale):
+        """Second half of `_step`: the corrector after the predictor's evaluation at t_next (`pending` from
+        `_step_predict`) or the Adams-Bashforth update, then the eps history."""
+        a_t, a_prev, s1m = self._coefs(index)
+        gs = float(guidance_scale)
         e_ts = []
-        if first:
-            assert len(first) == len(trajs), "trajectories must share their history length"
-            # pseudo improved Euler (plms.py:146-152): predictor, second evaluation at t_next
-            x0s = []
-            for tr, (e_c, e_u) in zip(trajs, evals):
-                x = tr.input["x"].float().contiguous()
-                x0s.append(x)
-                e_t = torch.empty_like(x)
-                x_pred = torch.empty_like(x)
-                ops.plms_update(x, e_c, e_u, gs, [], [1.0], a_t, a_prev, s1m, e_t, x_pred)
-                e_ts.append(e_t)
-                tr.input["x"] = x_pred
-                tr.input["timesteps"] = ts_next
-            evals2 = self._eval(trajs, uc, guidance_scale)
-            for tr, x, e_t, (e_c, e_u) in zip(trajs, x0s, e_ts, evals2):
+        if pending is not None:
+            x0s, e_ts = pending
+            for tr, x, e_t, (e_c, e_u) in zip(trajs, x0s, e_ts, evals):
                 x_prev = torch.empty_like(x)
                 ops.plms_update(x, e_c, e_u, gs, [e_t], [0.5, 0.5], a_t, a_prev, s1m, None, x_prev)
                 tr.input["x"] = x_prev

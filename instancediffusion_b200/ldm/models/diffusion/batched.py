@@ -1,0 +1,295 @@
+"""Many independent sampling requests advanced in lock step (not a reference module).
+
+A deployment that gets one layout per user would otherwise run one `sample()` call per request: every forward
+then has the batch of that one request (cond + uncond of one image: 512 GEMM rows at the 16x16 level against
+128-row tiles).  `sample_requests` evaluates, at every step, the live trajectories of all requests together in
+`forward_batched` chunks of up to `max_batch` images, each image with its own request's fuser scale (alpha
+schedule) and first-conv state.  Per request the arithmetic is that of its own sampler: the history and the
+PLMS updates are `PLMSBase._step_predict` / `_step_finish` on its own trajectories with its own guidance scale,
+and a Multi-instance request merges its latents with `ops.latent_mean` at its own step int(steps * mis), where
+steps is the length of the PLMS schedule (`schedule_steps`: S + 1 for some S, e.g. 31 for S = 30), as there.
+
+Contract: each returned latent equals, within floating-point tolerance, what `PLMSSampler.sample()` (input dict,
+mis = 0) or `PLMSSamplerInst.sample()` (input list [global, instance_1 .. instance_n]) returns for that request
+alone on the model in the state it had when `sample_requests` was called.  Afterwards the model's fuser scale and
+first-conv swap are what a sequential run of the same requests would leave.
+"""
+from __future__ import annotations
+
+from dataclasses import dataclass
+from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
+
+import numpy as np
+import torch
+
+from .... import ops
+from ...modules.attention import GatedSelfAttentionDense
+from ...modules.diffusionmodules.util import make_ddim_timesteps
+from ._plms_common import PLMSBase, Trajectory
+
+
+@dataclass
+class Request:
+    """One sampling request.  `input`: the dict `PLMSSampler.sample` takes, or the list [global, inst_1 .. inst_n]
+    of `PLMSSamplerInst.sample`; `shape`: (B, 4, H, W) of its latent (may be omitted when input x is given);
+    `mis`: the Multi-instance fraction (list inputs only).  `S`, if given, must equal the call's step count.
+    `mask` / `x0` (inpainting) are not supported and raise."""
+    input: Union[dict, List[dict]]
+    uc: Optional[torch.Tensor] = None
+    guidance_scale: float = 1.0
+    alpha_generator_func: Optional[Callable[[int], List[float]]] = None
+    mis: float = 0.0
+    shape: Optional[Tuple[int, ...]] = None
+    S: Optional[int] = None
+    mask: Optional[torch.Tensor] = None
+    x0: Optional[torch.Tensor] = None
+
+
+@dataclass(frozen=True)
+class RequestPlan:
+    """What the step planner needs of a request: trajectories before the merge (1 for plain PLMS), the step
+    before which they merge (None: never), images per trajectory and whether it evaluates cond + uncond."""
+    trajectories: int
+    merge_step: Optional[int]
+    images: int
+    cfg: bool
+
+    def live(self, step: int) -> int:
+        """Trajectories evaluated at `step`."""
+        return self.trajectories if self.merge_step is not None and step < self.merge_step else 1
+
+    def rows(self) -> int:
+        """Images one trajectory puts into a forward."""
+        return self.images * (2 if self.cfg else 1)
+
+
+def plan_chunks(slots: Sequence[Tuple[int, int]], plans: Sequence[RequestPlan], max_batch: int) -> List[List[Tuple[int, int]]]:
+    """Split (request, trajectory) slots, in order, into forward chunks of at most `max_batch` images.  A
+    trajectory's cond and uncond images stay in one chunk; a trajectory larger than `max_batch` gets a chunk
+    of its own."""
+    chunks, cur, used = [], [], 0
+    for r, k in slots:
+        n = plans[r].rows()
+        if cur and used + n > max_batch:
+            chunks.append(cur)
+            cur, used = [], 0
+        cur.append((r, k))
+        used += n
+    if cur:
+        chunks.append(cur)
+    return chunks
+
+
+def plan_step(plans: Sequence[RequestPlan], step: int, max_batch: int) -> List[List[Tuple[int, int]]]:
+    """Forward chunks of one evaluation at `step`: every live trajectory of every request."""
+    slots = [(r, k) for r, p in enumerate(plans) for k in range(p.live(step))]
+    return plan_chunks(slots, plans, max_batch)
+
+
+def _inputs_of(req: Request) -> List[dict]:
+    return req.input if isinstance(req.input, (list, tuple)) else [req.input]
+
+
+def schedule_steps(S: int, ddpm_timesteps: int = 1000) -> int:
+    """Steps of the PLMS schedule the samplers build for S (PLMSBase.make_schedule, 'uniform'): the timesteps
+    range(0, ddpm_timesteps, ddpm_timesteps // S), which is more than S when S does not divide ddpm_timesteps."""
+    return len(make_ddim_timesteps("uniform", int(S), int(ddpm_timesteps)))
+
+
+def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_timesteps: int = 1000) -> List[RequestPlan]:
+    """Validate the requests of one `sample_requests` call and describe them for the planner.  All must share the
+    step count S, the latent height x width and the context length; mask / x0 inpainting is not supported.
+    A Multi-instance request merges before step int(schedule_steps(S) * mis), as PLMSSamplerInst does."""
+    if not 0 < int(S) <= int(ddpm_timesteps):
+        raise ValueError(f"S must be in [1, {ddpm_timesteps}], got {S}")
+    steps = schedule_steps(S, ddpm_timesteps)
+    if int(max_batch) <= 0:
+        raise ValueError(f"max_batch must be positive, got {max_batch}")
+    if not requests:
+        raise ValueError("no requests")
+    plans, hw, ctx_len = [], None, None
+    for j, req in enumerate(requests):
+        if req.S is not None and int(req.S) != int(S):
+            raise ValueError(f"request {j}: S={req.S} differs from the call's S={S}")
+        if req.mask is not None or req.x0 is not None:
+            raise ValueError(f"request {j}: mask / x0 inpainting is not supported by sample_requests")
+        multi = isinstance(req.input, (list, tuple))
+        if not multi and req.mis != 0:
+            raise ValueError(f"request {j}: mis={req.mis} needs the input list [global, inst_1 .. inst_n]; "
+                             "a single input dict runs plain PLMS (mis = 0)")
+        if not 0 <= req.mis <= 1:
+            raise ValueError(f"request {j}: mis={req.mis} outside [0, 1]")
+        ins = _inputs_of(req)
+        if not ins:
+            raise ValueError(f"request {j}: empty input list")
+        shapes = {tuple(i["x"].shape) for i in ins if i.get("x") is not None}
+        if req.shape is not None:
+            shapes.add(tuple(req.shape))
+        if len(shapes) != 1:
+            raise ValueError(f"request {j}: latent shapes {sorted(shapes)} (give `shape` or one x shape for every input)")
+        shape = shapes.pop()
+        if len(shape) != 4:
+            raise ValueError(f"request {j}: latent shape {shape} is not (B, C, H, W)")
+        if hw is None:
+            hw = shape[2:]
+        elif shape[2:] != hw:
+            raise ValueError(f"request {j}: latent {shape[2]}x{shape[3]} differs from {hw[0]}x{hw[1]} of request 0")
+        for t in [i["context"] for i in ins] + ([req.uc] if req.uc is not None else []):
+            if ctx_len is None:
+                ctx_len = t.shape[1]
+            elif t.shape[1] != ctx_len:
+                raise ValueError(f"request {j}: context length {t.shape[1]} differs from {ctx_len}")
+        cfg = req.uc is not None and req.guidance_scale != 1
+        plans.append(RequestPlan(len(ins), int(steps * req.mis) if multi else None, shape[0], cfg))
+    return plans
+
+
+class _State:
+    """Per-request sampling state."""
+
+    def __init__(self, req: Request, plan: RequestPlan, S: int, device):
+        self.req, self.plan = req, plan
+        ins = _inputs_of(req)
+        if ins[0].get("x") is None:  # as the samplers: one noise tensor shared by every trajectory
+            img = torch.randn(tuple(req.shape), device=device)
+            for inp in ins:
+                inp["x"] = img
+        self.trajs = [Trajectory(inp) for inp in ins]
+        self.alphas = req.alpha_generator_func(S) if req.alpha_generator_func is not None else None
+        self.reached_zero = False
+        self.gs = float(req.guidance_scale)
+
+    def merge(self):
+        """Multi-instance merge: the global trajectory continues from the mean of the n+1 latents
+        (plms_instance.py:135)."""
+        xs = [tr.input["x"].float().contiguous() for tr in self.trajs]
+        merged = torch.empty_like(xs[0])
+        ops.latent_mean(xs, merged)
+        self.trajs[0].input["x"] = merged
+        self.trajs = self.trajs[:1]
+
+
+def _evaluate(model, states: List[_State], slots: List[Tuple[int, int]], max_batch: int, scales, restored, null_inputs):
+    """One UNet evaluation of the given trajectories, in forward chunks: {(request, trajectory): (e_c, e_u|None)}."""
+    plans = [s.plan for s in states]
+    out = {}
+    for chunk in plan_chunks(slots, plans, max_batch):
+        inputs, sc, rs = [], [], []
+        for r, k in chunk:
+            st = states[r]
+            tr = st.trajs[k]
+            inputs.append(tr.input)
+            if st.plan.cfg:
+                inputs.append(dict(x=tr.input["x"], timesteps=tr.input["timesteps"], context=st.req.uc,
+                                   grounding_input=null_inputs[r]))
+            n = 2 if st.plan.cfg else 1
+            sc += [scales[r]] * n
+            rs += [restored[r]] * n
+        outs = model.forward_batched(inputs, scales=sc, restored=rs)
+        j = 0
+        for r, k in chunk:
+            if states[r].plan.cfg:
+                out[(r, k)] = (outs[j], outs[j + 1])
+                j += 2
+            else:
+                out[(r, k)] = (outs[j], None)
+                j += 1
+    return out
+
+
+@torch.no_grad()
+def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], S: int, *,
+                    max_batch: int = 32) -> List[torch.Tensor]:
+    """Sample every request in `requests` (Request objects or dicts of its fields) with S PLMS steps; returns one
+    latent per request, in order.  `max_batch` bounds the images of one UNet forward.
+
+    The per-image fuser scales are those `utils.model.set_alpha_scale` sets (every gated fuser at the request's
+    alpha), and the model is left with that function's result for the last alpha of the last request that has an
+    alpha schedule.  Uncond images take the null grounding tokens of their own batch; where the grounding tokenizer
+    input was last prepared at a batch other than 1 and the request's, the request's own `sample()` would raise
+    instead ("grounding batch ... does not match latent batch")."""
+    from ....utils.model import set_alpha_scale
+    reqs = [r if isinstance(r, Request) else Request(**r) for r in requests]
+    plans = check_requests(reqs, S, max_batch, diffusion.num_timesteps)
+    base = PLMSBase(diffusion, model)
+    base.make_schedule(ddim_num_steps=S)
+    time_range = np.flip(base.ddim_timesteps)
+    total = base.ddim_timesteps.shape[0]
+    assert total == schedule_steps(S, diffusion.num_timesteps)
+    states = [_State(r, p, len(time_range), base.device) for r, p in zip(reqs, plans)]
+
+    fusers = [m for m in model.modules() if isinstance(m, GatedSelfAttentionDense)]
+    entry_scale = float(fusers[0].scale) if fusers else 0.0
+    if any(s.alphas is None for s in states) and any(float(f.scale) != entry_scale for f in fusers):
+        raise ValueError("requests without an alpha_generator_func run at the model's fuser scale, "
+                         "which differs between fusers")
+    entry_restored = bool(getattr(model, "_first_conv_restored", False))
+    # uncond inputs: the null grounding tokens of the request's batch (UNetModel.object_kv(None) uses the batch
+    # the grounding tokenizer input was last prepared with, which serves batch 1 and that batch)
+    gti = getattr(model, "grounding_tokenizer_input", None)
+    null_inputs = []
+    for p in plans:
+        own = gti is None or not getattr(gti, "set", False) or gti.batch in (1, p.images)
+        null_inputs.append(None if own else gti.get_null_input(batch=p.images))
+
+    # the model's hoisted-tensor caches must hold every input and every chunk combination of the run, or each
+    # forward recomputes its text / object K/V: raised for the run, restored afterwards
+    chunks = {tuple(c) for i in range(len(time_range)) for c in plan_step(plans, i, max_batch)}
+    bounds = {"hoist_cache_entries": sum(p.trajectories + 2 for p in plans) + 8, "cat_cache_entries": 2 * len(chunks) + 2}
+    saved = {k: model.__dict__[k] for k in bounds if k in model.__dict__}
+    for k, v in bounds.items():
+        setattr(model, k, max(v, getattr(model, k, 0)))
+    try:
+        _run(model, base, states, time_range, total, max_batch, entry_scale, entry_restored, null_inputs)
+    finally:
+        for k in bounds:
+            if k in saved:
+                setattr(model, k, saved[k])
+            else:
+                delattr(model, k)
+        model.trim_hoisted()  # the run's concatenations (hundreds of MB each) do not outlive it
+
+    for st in states:
+        if st.plan.merge_step == len(time_range):  # mis = 1: the merge follows the last step
+            st.merge()
+    # the model's fuser scale as a sequential run leaves it: the last alpha of the last request that sets one
+    for st in reversed(states):
+        if st.alphas is not None:
+            set_alpha_scale(model, st.alphas[-1])
+            break
+    return [st.trajs[0].input["x"] for st in states]
+
+
+def _run(model, base, states, time_range, total, max_batch, entry_scale, entry_restored, null_inputs):
+    """The S steps of sample_requests."""
+    for i in range(len(time_range)):
+        index = total - i - 1
+        scales, restored = [], []
+        for st in states:
+            if st.plan.merge_step == i:
+                st.merge()
+            alpha = st.alphas[i] if st.alphas is not None else entry_scale
+            if st.alphas is not None and alpha == 0 and not st.reached_zero:
+                st.reached_zero = True
+                model.restore_first_conv_from_SD()  # the swap a run of this request makes here (PLMSBase._set_alpha)
+            scales.append(float(alpha))
+        model_restored = bool(getattr(model, "_first_conv_restored", False))
+        for st in states:
+            restored.append(entry_restored or (st.reached_zero and model_restored))
+        steps = {}
+        for r, st in enumerate(states):
+            ts, ts_next = base._timesteps(st.plan.images, i, time_range)
+            steps[r] = ts_next
+            for tr in st.trajs:
+                tr.input["timesteps"] = ts
+        slots = [(r, k) for r, st in enumerate(states) for k in range(len(st.trajs))]
+        evals = _evaluate(model, states, slots, max_batch, scales, restored, null_inputs)
+        pending = {}
+        for r, st in enumerate(states):
+            pending[r] = base._step_predict(st.trajs, [evals[(r, k)] for k in range(len(st.trajs))], steps[r], index,
+                                            st.gs)
+        again = [(r, k) for r, k in slots if pending[r] is not None]
+        if again:  # first step of a trajectory: the corrector's evaluation at t_next
+            evals.update(_evaluate(model, states, again, max_batch, scales, restored, null_inputs))
+        for r, st in enumerate(states):
+            base._step_finish(st.trajs, [evals[(r, k)] for k in range(len(st.trajs))], pending[r], index, st.gs)

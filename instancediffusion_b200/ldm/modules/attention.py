@@ -80,12 +80,14 @@ class FeedForward(PackedModule):
     def _pack(self):
         return {"w2": w16(self.net[2].weight), "b2": f32(self.net[2].bias)}
 
-    def _fwd(self, x16, residual=None, gate=1.0, out=None, ln=None, want_stats=False):
+    def _fwd(self, x16, residual=None, gate=1.0, out=None, ln=None, want_stats=False, gate_rows=None, rows_per_batch=0):
         """x16: LayerNorm-ed input (or, with ln=(RowStats, LnFold), the stream itself).  Returns residual +
-        gate * FF(x16) (or FF(x16) without residual); with want_stats also the RowStats of the result."""
+        gate * FF(x16) (or FF(x16) without residual); with want_stats also the RowStats of the result.
+        gate_rows: fp32 per-image factor of the gate (images of rows_per_batch rows), see ops.gemm."""
         p = self.pk()
         h = self.net[0]._fwd(x16, ln=ln)
-        return ops.gemm(h, p["w2"], p["b2"], residual=residual, gate=gate, out=out, want_stats=want_stats)
+        return ops.gemm(h, p["w2"], p["b2"], residual=residual, gate=gate, out=out, want_stats=want_stats,
+                        gate_rows=gate_rows, rows_per_batch=rows_per_batch)
 
     def forward(self, x):
         x16, B, N = to_tokens(x)
@@ -178,9 +180,10 @@ class SelfAttention(PackedModule):
         return ops.gemm(x16, wkv)
 
     def _fwd(self, x16, B, N, residual=None, gate=1.0, extra_kv=None, n_extra=0, extra_batch=0, out=None, ln=None,
-             want_stats=False, mask=None):
+             want_stats=False, mask=None, gate_rows=None):
         """x16: normalised tokens [B*N, C] -- or, with ln=(RowStats, LnFold), the un-normalised stream.
-        extra_kv: [Be*n_extra, 2C] additional keys/values (the object tokens of the gated block)."""
+        extra_kv: [Be*n_extra, 2C] additional keys/values (the object tokens of the gated block).
+        gate_rows: fp32 [B] per-image factor of the residual gate (ops.gemm)."""
         p = self.pk()
         C = self.heads * self.dim_head
         if ln is not None:
@@ -195,7 +198,8 @@ class SelfAttention(PackedModule):
             kw["mask"] = mask
         a = ops.attention(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], batch=B, heads=self.heads,
                           head_dim=self.dim_head, nq=N, n0=N, scale=self.scale, **kw)
-        return ops.gemm(a, p["wo"], p["bo"], residual=residual, gate=gate, out=out, want_stats=want_stats)
+        return ops.gemm(a, p["wo"], p["bo"], residual=residual, gate=gate, out=out, want_stats=want_stats,
+                        gate_rows=gate_rows, rows_per_batch=N if gate_rows is not None else 0)
 
     def forward(self, x, grounding_input=None, drop_box_mask=False):
         x16, B, N = to_tokens(x)
@@ -244,17 +248,23 @@ class GatedSelfAttentionDense(PackedModule):
         where the visual tokens are the 64x64 grid (N + n_obj - 4 * n_inst - 64 == 64 * 64)."""
         return (not self.attn.efficient_attention) and N + n_obj - 4 * n_inst - 64 == 64 * 64
 
-    def _fwd(self, x16, stats, B, N, obj_kv, n_obj, obj_batch, mask=None):
+    def _fwd(self, x16, stats, B, N, obj_kv, n_obj, obj_batch, mask=None, scale=None):
         """In-place on x16 (the residual stream; `stats` = its RowStats).  Returns (x16, stats).  Identity
-        when scale == 0 (the alpha=0 steps).  mask: (mask_q, mask_k) words of ops.attmask_words or None."""
-        if self.scale == 0:
+        when scale == 0 (the alpha=0 steps).  mask: (mask_q, mask_k) words of ops.attmask_words or None.
+        scale: None (this module's `.scale`), a float, or an fp32 [B] tensor of per-image scales (batched requests
+        at different alpha steps: the gates become tanh(alpha) * scale[b]; rows with scale 0 pass unchanged)."""
+        if scale is None:
+            scale = self.scale
+        rows = scale if isinstance(scale, torch.Tensor) else None
+        if rows is None and scale == 0:
             return x16, stats
         p = self.pk()
-        x16, stats = self.attn._fwd(x16, B, N, residual=x16, gate=float(self.scale) * p["tanh_attn"],
+        s = 1.0 if rows is not None else float(scale)
+        x16, stats = self.attn._fwd(x16, B, N, residual=x16, gate=s * p["tanh_attn"],
                                     extra_kv=obj_kv, n_extra=n_obj, extra_batch=obj_batch, out=x16,
-                                    ln=(stats, p["qkv"]), want_stats=True, mask=mask)
-        return self.ff._fwd(x16, residual=x16, gate=float(self.scale) * p["tanh_dense"], out=x16,
-                            ln=(stats, p["ff"]), want_stats=True)
+                                    ln=(stats, p["qkv"]), want_stats=True, mask=mask, gate_rows=rows)
+        return self.ff._fwd(x16, residual=x16, gate=s * p["tanh_dense"], out=x16,
+                            ln=(stats, p["ff"]), want_stats=True, gate_rows=rows, rows_per_batch=N if rows is not None else 0)
 
     def forward(self, x, objs, grounding_input=None, drop_box_mask=False):
         x16, B, N = to_tokens(x)
@@ -308,12 +318,13 @@ class BasicTransformerBlock(PackedModule):
             "ff": self.ff.net[0].fold(self.norm3),
         }
 
-    def _fwd(self, x16, stats, B, N, ctx_kv, M, obj_kv, n_obj, obj_batch, mask=None):
+    def _fwd(self, x16, stats, B, N, ctx_kv, M, obj_kv, n_obj, obj_batch, mask=None, fuser_scale=None):
         """x16: the residual stream (updated in place), stats: its RowStats (from the GEMM that wrote it).
-        mask: instance-isolation mask words for the fuser (64x64 level, efficient_attention=False) or None."""
+        mask: instance-isolation mask words for the fuser (64x64 level, efficient_attention=False) or None.
+        fuser_scale: overrides the fuser's `.scale` (GatedSelfAttentionDense._fwd `scale`)."""
         p = self.pk()
         x16, stats = self.attn1._fwd(x16, B, N, residual=x16, out=x16, ln=(stats, p["qkv1"]), want_stats=True)
-        x16, stats = self.fuser._fwd(x16, stats, B, N, obj_kv, n_obj, obj_batch, mask=mask)
+        x16, stats = self.fuser._fwd(x16, stats, B, N, obj_kv, n_obj, obj_batch, mask=mask, scale=fuser_scale)
         x16, stats = self.attn2._fwd(x16, ctx_kv, B, N, M, residual=x16, out=x16, ln=(stats, p["q2"]), want_stats=True)
         return self.ff._fwd(x16, residual=x16, out=x16, ln=(stats, p["ff"]))
 
@@ -360,8 +371,9 @@ class SpatialTransformer(PackedModule):
             "w_out": pack_conv1x1(w16(self.proj_out.weight)), "b_out": f32(self.proj_out.bias),
         }
 
-    def _fwd(self, x16, B, H, W, ctx_kvs, M, obj_kvs, n_obj, obj_batch, mask=None):
-        """x16 fp16 [B*H*W, C].  ctx_kvs / obj_kvs: one entry per transformer block.  mask: see BasicTransformerBlock."""
+    def _fwd(self, x16, B, H, W, ctx_kvs, M, obj_kvs, n_obj, obj_batch, mask=None, fuser_scale=None):
+        """x16 fp16 [B*H*W, C].  ctx_kvs / obj_kvs: one entry per transformer block.  mask, fuser_scale: see
+        BasicTransformerBlock."""
         p = self.pk()
         n = ops.groupnorm(x16, p["gn_g"], p["gn_b"], batch=B, hw=H * W, groups=32, eps=self.norm.eps, silu=False)
         t, stats = ops.gemm(n, p["w_in"], p["b_in"], want_stats=True)
@@ -369,7 +381,7 @@ class SpatialTransformer(PackedModule):
             if i > 0:  # (depth > 1: the previous block's FF out-projection did not keep statistics)
                 stats = ops.row_stats(t)
             t = blk._fwd(t, stats, B, H * W, ctx_kvs[i], M, obj_kvs[i] if obj_kvs is not None else None, n_obj, obj_batch,
-                         mask=mask if H * W == 64 * 64 else None)
+                         mask=mask if H * W == 64 * 64 else None, fuser_scale=fuser_scale)
         return ops.gemm(t, p["w_out"], p["b_out"], residual=x16)
 
     def forward(self, x, context, objs, grounding_input=None, drop_box_mask=False):

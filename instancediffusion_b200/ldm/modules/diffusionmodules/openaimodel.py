@@ -221,6 +221,11 @@ class ResBlock(TimestepBlock):
 
 
 class UNetModel(PackedModule):
+    # bounds of the hoisted-tensor caches: text K/V and object K/V entries (one per distinct input), concatenations
+    # (one per combination of inputs in a batched forward); a cache that reaches its bound is cleared
+    hoist_cache_entries = 64
+    cat_cache_entries = 6
+
     def __init__(self, image_size, in_channels, model_channels, out_channels, num_res_blocks,
                  attention_resolutions, dropout=0, channel_mult=(1, 2, 4, 8), conv_resample=True, dims=2,
                  use_checkpoint=False, num_heads=8, use_scale_shift_norm=False, transformer_depth=1,
@@ -331,6 +336,11 @@ class UNetModel(PackedModule):
             return
         if getattr(self, "_first_conv_restored", False):
             return
+        self.set_sd_first_conv(self.load_sd_first_conv())
+
+    def load_sd_first_conv(self) -> Dict[str, torch.Tensor]:
+        """The SD1.5 input-conv state dict restore_first_conv_from_SD swaps in, read from pretrained/ (cwd-relative
+        as in the reference, openaimodel.py:476) or $IDIFF_PRETRAINED_DIR.  Swaps nothing."""
         name = "SD_v1_5_input_conv_weight_bias.pth" if self.sd_v1_5 else "SD_input_conv_weight_bias.pth"
         path = os.path.join("pretrained", name)
         if not os.path.exists(path):
@@ -341,7 +351,7 @@ class UNetModel(PackedModule):
                 raise FileNotFoundError(
                     f"{path} not found (cwd-relative as in the reference, openaimodel.py:476); "
                     "set IDIFF_PRETRAINED_DIR or call set_sd_first_conv(state_dict)")
-        self.set_sd_first_conv(torch.load(path, map_location="cpu"))
+        return torch.load(path, map_location="cpu")
 
     def set_sd_first_conv(self, sd_weights: Dict[str, torch.Tensor]):
         conv = self.input_blocks[0][0]
@@ -369,13 +379,24 @@ class UNetModel(PackedModule):
             self.input_blocks[0][0] = conv.to(self.input_blocks[0][0].weight.device)
             self._first_conv_restored = False
 
-    def _in_conv_pack(self):
-        key = bool(getattr(self, "_first_conv_restored", False))
+    def _in_conv_pack(self, restored: Optional[bool] = None):
+        """Packed input conv of the model's current first-conv state, or (restored=True / False) of the SD1.5 /
+        the model's own conv whatever the current state is.  The SD weights are the ones last given to
+        set_sd_first_conv, else load_sd_first_conv()."""
+        cur = bool(getattr(self, "_first_conv_restored", False))
+        key = cur if restored is None else bool(restored)
         hit = self._in_packs.get(key)
         if hit is None:
             conv0 = self.input_blocks[0][0]
+            if key == cur:
+                w, b = conv0.weight, conv0.bias
+            else:
+                sd = self.first_conv_state_dict if cur else getattr(self, "_sd_conv_src", None)
+                if sd is None:
+                    sd = self.load_sd_first_conv()
+                w, b = sd["weight"].to(conv0.weight.device), sd["bias"].to(conv0.weight.device)
             with torch.no_grad():
-                hit = (_pack_conv3x3_padded(conv0.weight, 64), f32(conv0.bias))
+                hit = (_pack_conv3x3_padded(w, 64), f32(b))
             self._in_packs[key] = hit
         return hit
 
@@ -460,7 +481,7 @@ class UNetModel(PackedModule):
         p = self.pk()
         c16 = context.reshape(-1, context.shape[-1]).to(half()).contiguous()
         kv = ops.gemm(c16, p["w_ctx_all"])
-        if len(self._ctx_cache) > 64:
+        if len(self._ctx_cache) > self.hoist_cache_entries:
             self._ctx_cache.clear()
             self._cat_cache.clear()
         self._ctx_cache[key] = (context, kv)  # keep `context` alive so the key stays unique
@@ -489,7 +510,7 @@ class UNetModel(PackedModule):
         blocks = [blk for st in self._transformers() for blk in st.transformer_blocks]
         kvs = [blk.fuser.project_objs(objs16) for blk in blocks]
         mask = attention_mask_words(blocks[0].fuser, gi, drop_box_mask, Bo, 64 * 64, n_obj)
-        if len(self._obj_cache) > 64:
+        if len(self._obj_cache) > self.hoist_cache_entries:
             self._obj_cache.clear()
             self._cat_cache.clear()
         val = (kvs, Bo, n_obj, mask)
@@ -503,6 +524,15 @@ class UNetModel(PackedModule):
         self._obj_cache.clear()
         self._cat_cache.clear()
 
+    def trim_hoisted(self):
+        """Drop the batch concatenations of the hoisted tensors, and the per-input caches where they hold more
+        entries than their bound (a run with raised bounds leaves them so)."""
+        self._cat_cache.clear()
+        if len(self._ctx_cache) > self.hoist_cache_entries:
+            self._ctx_cache.clear()
+        if len(self._obj_cache) > self.hoist_cache_entries:
+            self._obj_cache.clear()
+
     def clear_caches(self):
         self.clear_hoisted()
         self._graphs.clear()
@@ -514,9 +544,12 @@ class UNetModel(PackedModule):
         return any(blk.fuser.scale != 0 for st in self._transformers() for blk in st.transformer_blocks)
 
     def _core(self, x: torch.Tensor, t: torch.Tensor, ctx_kv_all: torch.Tensor, M: int,
-              obj_kvs: Optional[List[torch.Tensor]], n_obj: int, mask=None) -> torch.Tensor:
+              obj_kvs: Optional[List[torch.Tensor]], n_obj: int, mask=None, fuser_scale=None,
+              n_restored: Optional[int] = None) -> torch.Tensor:
         """x fp32 (B,4,H,W), t fp32 (B,), ctx_kv_all fp16 [B*M, sumKV], obj_kvs per-fuser [B*n_obj, 2C]
-        (or None on alpha=0 steps) -> eps fp32 (B,4,H,W)."""
+        (or None on alpha=0 steps) -> eps fp32 (B,4,H,W).  fuser_scale: None (each fuser's `.scale`), a float or
+        an fp32 [B] tensor of per-image scales.  n_restored: None (the model's first-conv state for every image) or
+        the number of trailing images that take the SD1.5 input conv, the others the model's own."""
         p = self.pk()
         B, _, H, W = x.shape
         # time embedding (openaimodel.py:497-498) ; SiLU of emb_layers[0] folded into the last epilogue
@@ -538,7 +571,8 @@ class UNetModel(PackedModule):
                 ctx_kvs.append(ctx_kv_all[:, a:b])
                 okvs.append(obj_kvs[blk_idx[0]] if obj_kvs is not None else None)
                 blk_idx[0] += 1
-            return st._fwd(h, B, hh, ww, ctx_kvs, M, okvs if obj_kvs is not None else None, n_obj, B, mask=mask)
+            return st._fwd(h, B, hh, ww, ctx_kvs, M, okvs if obj_kvs is not None else None, n_obj, B, mask=mask,
+                           fuser_scale=fuser_scale)
 
         def run_block(seq, h, hh, ww):
             for layer in seq:
@@ -557,8 +591,15 @@ class UNetModel(PackedModule):
             return h, hh, ww
 
         x16 = ops.nchw_f32_to_nhwc_f16(x, 64)
-        w_in, b_in = self._in_conv_pack()
-        h = ops.gemm(x16, w_in, b_in, conv=(B, H, W, 64))
+        if n_restored is None or n_restored in (0, B):
+            w_in, b_in = self._in_conv_pack(None if n_restored is None else n_restored == B)
+            h = ops.gemm(x16, w_in, b_in, conv=(B, H, W, 64))
+        else:  # one conv GEMM per first-conv state, each on its contiguous range of images
+            h = torch.empty((B * H * W, self.model_channels), dtype=half(), device=x.device)
+            for b0, nb, restored in ((0, B - n_restored, False), (B - n_restored, n_restored, True)):
+                w_in, b_in = self._in_conv_pack(restored)
+                rows = slice(b0 * H * W, (b0 + nb) * H * W)
+                ops.gemm(x16[rows], w_in, b_in, conv=(nb, H, W, 64), out=h[rows])
         hh, ww = H, W
         hs = [(h, hh, ww)]
         for module in list(self.input_blocks)[1:]:
@@ -582,13 +623,15 @@ class UNetModel(PackedModule):
         ops.gemm(h, p["w_out"], p["cb_out"], conv=(B, hh, ww, self.model_channels), out_nchw=eps)
         return eps
 
-    def _gather_inputs(self, inputs: List[dict]):
+    def _gather_inputs(self, inputs: List[dict], active: Optional[bool] = None):
         """Concatenate independent forwards (cond / uncond / MIS trajectories) along the batch.  The step-invariant
         parts -- text K/V, per-fuser object K/V, mask words -- are concatenated once per combination of inputs and
         reused on every later step (the same tensor objects come back, which lets `_CoreGraph.replay` skip its copies
-        as well): 17-19 torch.cat launches and as many copies per forward otherwise."""
+        as well): 17-19 torch.cat launches and as many copies per forward otherwise.  active: whether the fusers run
+        (default: any fuser has a non-zero `.scale`)."""
         xs, ts, ctxs, okv_lists, masks, bs = [], [], [], [], [], []
-        active = self._fusers_active()
+        if active is None:
+            active = self._fusers_active()
         n_obj = 0
         for inp in inputs:
             x = inp["x"]
@@ -642,37 +685,75 @@ class UNetModel(PackedModule):
                     mqs.append(mq if mq.shape[0] == b else mq.expand(b, -1))
                     mks.append(mk if mk.shape[0] == b else mk.expand(b, -1))
             mask = (torch.cat(mqs, 0).contiguous(), torch.cat(mks, 0).contiguous())
-        if len(self._cat_cache) >= 6:  # (an entry holds the concatenated text K/V: tens of MB to ~1 GB at MIS batch sizes)
+        if len(self._cat_cache) >= self.cat_cache_entries:  # (an entry holds the concatenated text K/V: tens of MB to ~1 GB at MIS batch sizes)
             self._cat_cache.clear()
         keep = (ctxs, [k for k, _ in okv_lists], [m for m, _ in masks])  # keeps the keyed objects (and their ids) alive
         self._cat_cache[key] = (keep, ctx, okv, mask)
         return x, t, ctx, M, okv, n_obj, mask
 
     @torch.no_grad()
-    def forward_batched(self, inputs: List[dict]) -> List[torch.Tensor]:
-        """Run several independent forwards as one batch; returns one eps tensor per input."""
+    def forward_batched(self, inputs: List[dict], *, scales: Optional[List[float]] = None,
+                        restored: Optional[List[bool]] = None) -> List[torch.Tensor]:
+        """Run several independent forwards as one batch; returns one eps tensor per input.
+
+        scales: one fuser scale per input -- what set_alpha_scale would set for a forward of that input alone --
+        instead of the fusers' own `.scale`.  Equal scales run the scalar-gate path (all 0: the fusers are skipped);
+        mixed scales run the fusers on every image with the gates tanh(alpha) * scale of each image.
+        restored: per input, True = the SD1.5 input conv that restore_first_conv_from_SD swaps in, False = the
+        model's own; the model's conv is not swapped.  Default: the model's current first-conv state."""
         if getattr(self, "_storage_epoch", None) != ops.STORAGE_EPOCH:  # storage type switched: derived tensors are stale
             self._drop_derived()
             self._storage_epoch = ops.STORAGE_EPOCH
-        x, t, ctx, M, okv, n_obj, mask = self._gather_inputs(inputs)
-        eps = self._run_core(x, t, ctx, M, okv, n_obj, mask)
+        n = len(inputs)
+        for arg, name in ((scales, "scales"), (restored, "restored")):
+            if arg is not None and len(arg) != n:
+                raise ValueError(f"forward_batched: {len(arg)} {name} for {n} inputs")
         sizes = [inp["x"].shape[0] for inp in inputs]
-        return list(torch.split(eps, sizes, 0))
+        if restored is None:
+            order = list(range(n))
+            n_restored = sum(sizes) if getattr(self, "_first_conv_restored", False) else 0
+        else:  # images of the SD1.5 conv last: each input conv is one GEMM over a contiguous range of images
+            order = [i for i in range(n) if not restored[i]] + [i for i in range(n) if restored[i]]
+            n_restored = sum(sizes[i] for i in range(n) if restored[i])
+        ins = [inputs[i] for i in order]
+        fuser_scale, active = None, None
+        if scales is not None:
+            s = [float(scales[i]) for i in order]
+            if all(v == s[0] for v in s):
+                fuser_scale, active = s[0], s[0] != 0
+            else:
+                rows = torch.tensor([v for v, i in zip(s, order) for _ in range(sizes[i])], dtype=torch.float32)
+                fuser_scale, active = rows.pin_memory().to(ins[0]["x"].device, non_blocking=True), True
+        x, t, ctx, M, okv, n_obj, mask = self._gather_inputs(ins, active)
+        eps = self._run_core(x, t, ctx, M, okv, n_obj, mask, fuser_scale, n_restored)
+        outs = torch.split(eps, [sizes[i] for i in order], 0)
+        res = [None] * n
+        for j, i in enumerate(order):
+            res[i] = outs[j]
+        return res
 
-    def _run_core(self, x, t, ctx, M, okv, n_obj, mask=None):
+    def _run_core(self, x, t, ctx, M, okv, n_obj, mask=None, fuser_scale=None, n_restored=None):
         if not self.use_cuda_graph:
-            return self._core(x, t, ctx, M, okv, n_obj, mask)
+            return self._core(x, t, ctx, M, okv, n_obj, mask, fuser_scale, n_restored)
         # the fuser gates scale*tanh(alpha) are kernel arguments, frozen into a captured graph: the
         # per-fuser scales (set_alpha_scale may set any value, alpha_generator's decay stage is
-        # fractional) are part of the key
-        scales = tuple(float(blk.fuser.scale) for st in self._transformers() for blk in st.transformer_blocks) \
-            if okv is not None else ()
-        key = (tuple(x.shape), M, scales, n_obj, mask is not None, getattr(self, "_first_conv_restored", False))
+        # fractional) are part of the key.  Per-image scales are a static input buffer of the graph instead.
+        if okv is None:
+            scales = ()
+        elif isinstance(fuser_scale, torch.Tensor):
+            scales = ("per-image",)
+        else:
+            scales = tuple(float(blk.fuser.scale if fuser_scale is None else fuser_scale)
+                           for st in self._transformers() for blk in st.transformer_blocks)
+        if n_restored is None:
+            n_restored = x.shape[0] if getattr(self, "_first_conv_restored", False) else 0
+        # (set_sd_first_conv drops the graphs whose last key entry, the count of SD-conv images, is non-zero)
+        key = (tuple(x.shape), M, scales, n_obj, mask is not None, n_restored)
         g = self._graphs.get(key)
         if g is None:
-            g = _CoreGraph(self, x, t, ctx, M, okv, n_obj, mask)
+            g = _CoreGraph(self, x, t, ctx, M, okv, n_obj, mask, fuser_scale, n_restored)
             self._graphs[key] = g
-        return g.replay(x, t, ctx, okv, mask)
+        return g.replay(x, t, ctx, okv, mask, fuser_scale)
 
     def forward_single_input(self, input):
         return self.forward_batched([input])[0]
@@ -685,12 +766,14 @@ class _CoreGraph:
     """One captured CUDA graph of UNetModel._core for a fixed (batch, shapes, fuser on/off) key.
     Inputs are copied into static buffers, the graph is replayed, the static output is cloned."""
 
-    def __init__(self, model: UNetModel, x, t, ctx, M, okv, n_obj, mask=None):
+    def __init__(self, model: UNetModel, x, t, ctx, M, okv, n_obj, mask=None, fuser_scale=None, n_restored=None):
         self.x = x.clone()
         self.t = t.clone()
         self.ctx = ctx.clone()
         self.okv = [o.clone() for o in okv] if okv is not None else None
         self.mask = (mask[0].clone(), mask[1].clone()) if mask is not None else None
+        # per-image fuser scales: a static input like x and t (a float or None is part of the graph key)
+        self.scale = fuser_scale.clone() if isinstance(fuser_scale, torch.Tensor) else fuser_scale
         model.pk()  # make sure packing (allocations + host work) happens outside capture
         for st in model._transformers():
             st.pk()
@@ -706,15 +789,17 @@ class _CoreGraph:
             s = torch.cuda.Stream()
             s.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(s):
-                model._core(self.x, self.t, self.ctx, M, self.okv, n_obj, self.mask)
+                model._core(self.x, self.t, self.ctx, M, self.okv, n_obj, self.mask, self.scale, n_restored)
             torch.cuda.current_stream().wait_stream(s)
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.graph):
-                self.out = model._core(self.x, self.t, self.ctx, M, self.okv, n_obj, self.mask)
+                self.out = model._core(self.x, self.t, self.ctx, M, self.okv, n_obj, self.mask, self.scale, n_restored)
 
-    def replay(self, x, t, ctx, okv, mask=None):
+    def replay(self, x, t, ctx, okv, mask=None, fuser_scale=None):
         self.x.copy_(x)
         self.t.copy_(t)
+        if isinstance(self.scale, torch.Tensor):
+            self.scale.copy_(fuser_scale)
         # step-invariant inputs: the static buffers already hold them when the very same (immutable, cached)
         # tensor objects come back -- every step of a sampling run after the first
         last = getattr(self, "_last", (None, None, None))

@@ -196,11 +196,14 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
          geglu: bool = False, silu: bool = False, gelu: bool = False,
          conv: Optional[Tuple[int, int, int, int]] = None,
          out_nchw: Optional[torch.Tensor] = None,
-         ln: Optional[Tuple["RowStats", torch.Tensor, float]] = None, want_stats: bool = False):
+         ln: Optional[Tuple["RowStats", torch.Tensor, float]] = None, want_stats: bool = False,
+         gate_rows: Optional[torch.Tensor] = None):
     """out = epilogue(a @ w.T).  a: fp16 [M,K] (or NHWC [B,H,W,Cin] flattened with conv=(B,H,W,Cin));
     w: fp16 [N,K].  See idiff_gemm in include/idiff_b200.h.
     ln = (RowStats of a's rows, colsum, eps): a is the un-normalised stream and w / bias are LayerNorm-folded
-    (fold_layernorm).  want_stats: also return the RowStats of the output rows -> (out, stats)."""
+    (fold_layernorm).  want_stats: also return the RowStats of the output rows -> (out, stats).
+    gate_rows: fp32 [batch entries] (entry = row // rows_per_batch, conv: the image) multiplying `gate` per
+    entry: out = residual + gate * gate_rows[b] * (...).  Needs `residual`."""
     lib = _lib.load()
     _req(a, HALF, "a")
     _req(w, HALF, "w")
@@ -248,6 +251,13 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
         args.ldr = residual.stride(0)
     args.residual = _ptr(residual)
     args.gate = float(gate)
+    if gate_rows is not None:
+        _req(gate_rows, torch.float32, "gate_rows")
+        entries = conv[0] if conv is not None else -(-M // (rows_per_batch if rows_per_batch > 0 else M))
+        if residual is None or not gate_rows.is_contiguous() or gate_rows.numel() < entries:
+            raise _lib.IdiffError(f"gemm: gate_rows needs a residual and {entries} contiguous entries "
+                                  f"(got {tuple(gate_rows.shape)})")
+        args.gate_b = gate_rows.data_ptr()
     args.workspace, args.workspace_bytes = _gemm_workspace(a.device)
     args.M, args.N, args.K = M, N, K
     args.lda, args.ldw = lda, w.stride(0)
