@@ -216,6 +216,17 @@ int idiff_plms_update(const float* x, const float* e_c, const float* e_u, float 
 int idiff_latent_mean(const float* const* xs_dev, int count, float* out, long n, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * idiff_conv_in_select: the UNet's input conv (3x3, padding 1, 4 -> cout channels) with one of two
+ * weight sets per image: the model's own or the SD1.5 conv that openaimodel.py:469-480 swaps in.
+ *   out[b, y, x, n] = bias_s[n] + sum_{ky,kx,c} w_s[(ky*3 + kx)*4 + c][n] * x16[b, c, y+ky-1, x+kx-1]
+ * s = flags[b] (0: w0/b0, else w1/b1; int32 in device memory), x16 = x rounded to the storage type
+ * (zero outside the image), fp32 accumulation.  x fp32 NCHW (B, 4, H, W); w 16-bit [36, cout]
+ * (tap-major, then input channel); b fp32 [cout]; out 16-bit NHWC [B*H*W, cout].  cout even, <= 1024.
+ * ------------------------------------------------------------------------------------------- */
+int idiff_conv_in_select(const float* x, const void* w0, const float* b0, const void* w1, const float* b1,
+                         const int* flags, void* out, int batch, int h, int w, int cout, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Instance-isolation attention mask, host prep on the GPU
  * ------------------------------------------------------------------------------------------- */
 /* utils/input.py:34-37,79 (get_attmask_w_box): att_masks[b, k, x1:x2, y1:y2] = 1 for every instance k < counts[b]

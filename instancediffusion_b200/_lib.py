@@ -78,6 +78,7 @@ SIGNATURES = {
     "idiff_fourier_embed": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "idiff_plms_update": (_i, [_vp, _vp, _vp, _f, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _f, _vp, _vp, _l, _vp]),
     "idiff_latent_mean": (_i, [_vp, _i, _vp, _l, _vp]),
+    "idiff_conv_in_select": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "idiff_timestep_embedding": (_i, [_vp, _vp, _i, _i, _vp]),
     "idiff_silu_f16": (_i, [_vp, _vp, _l, _vp]),
     "idiff_segs_inconv": (_i, [_vp, C.POINTER(C.c_long), _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),

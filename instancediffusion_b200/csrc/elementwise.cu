@@ -193,6 +193,66 @@ __global__ void latent_mean_kernel(const float* const* __restrict__ xs, int coun
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// input conv of the UNet (openaimodel.py:469-480) with the conv chosen per image: 3x3, padding 1,
+// 4 -> cout channels.  One CTA per CONV_IN_ROWS output rows of one image, one thread per channel
+// pair: the thread keeps its 2 x 36 weights in registers and walks the rows, reading the 3x3x4
+// neighbourhood of each pixel from a shared tile of storage-rounded inputs.
+// ---------------------------------------------------------------------------------------------
+constexpr int CONV_IN_ROWS = 4;
+
+__global__ void __launch_bounds__(512)
+conv_in_select_kernel(const float* __restrict__ x, const h16* __restrict__ w0, const float* __restrict__ b0,
+                      const h16* __restrict__ w1, const float* __restrict__ b1, const int* __restrict__ flags,
+                      uint32_t* __restrict__ out, int H, int W, int cout) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ float4 tile[];  // [(CONV_IN_ROWS + 2) * (W + 2)], channels of one pixel in one float4
+  const int b = blockIdx.y, y0 = blockIdx.x * CONV_IN_ROWS;
+  const int TW = W + 2;
+  const long plane = (long)H * W;
+  const float* xb = x + (long)b * 4 * plane;
+  for (int i = threadIdx.x; i < (CONV_IN_ROWS + 2) * TW; i += blockDim.x) {
+    const int iy = y0 - 1 + i / TW, ix = i % TW - 1;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
+      const long p = (long)iy * W + ix;  // x rounded to the storage type, as the GEMM path reads it
+      v = make_float4(h2f(f2h(xb[p])), h2f(f2h(xb[plane + p])), h2f(f2h(xb[2 * plane + p])),
+                      h2f(f2h(xb[3 * plane + p])));
+    }
+    tile[i] = v;
+  }
+  const bool sd = flags[b] != 0;
+  const h16* w = sd ? w1 : w0;
+  const int c0 = 2 * threadIdx.x;
+  float2 wr[36];
+#pragma unroll
+  for (int k = 0; k < 36; ++k)
+    wr[k] = unpack_half2(*reinterpret_cast<const uint32_t*>(w + (long)k * cout + c0));
+  const float2 bias = *reinterpret_cast<const float2*>((sd ? b1 : b0) + c0);
+  __syncthreads();
+  const int rows = min(CONV_IN_ROWS, H - y0);
+  for (int r = 0; r < rows; ++r) {
+    uint32_t* orow = out + ((long)b * plane + (long)(y0 + r) * W) * (cout / 2) + threadIdx.x;
+    for (int px = 0; px < W; ++px) {
+      float a0 = 0.f, a1 = 0.f;
+#pragma unroll
+      for (int ky = 0; ky < 3; ++ky) {
+#pragma unroll
+        for (int kx = 0; kx < 3; ++kx) {
+          const float4 v = tile[(r + ky) * TW + px + kx];
+          const float2* wk = wr + (ky * 3 + kx) * 4;
+          a0 = fmaf(wk[0].x, v.x, a0); a1 = fmaf(wk[0].y, v.x, a1);
+          a0 = fmaf(wk[1].x, v.y, a0); a1 = fmaf(wk[1].y, v.y, a1);
+          a0 = fmaf(wk[2].x, v.z, a0); a1 = fmaf(wk[2].y, v.z, a1);
+          a0 = fmaf(wk[3].x, v.w, a0); a1 = fmaf(wk[3].y, v.w, a1);
+        }
+      }
+      orow[(long)px * (cout / 2)] = pack_half2(a0 + bias.x, a1 + bias.y);
+    }
+  }
+}
+
 __global__ void silu_f16_kernel(const h16* __restrict__ x, h16* __restrict__ y, long n) {
   pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
   pdl_wait();               // ... and this one touches global memory only after its predecessor finished
@@ -348,6 +408,21 @@ extern "C" int idiff_plms_update(const float* x, const float* e_c, const float* 
 extern "C" int idiff_latent_mean(const float* const* xs_dev, int count, float* out, long n, void* stream) {
   IDIFF_REQUIRE(xs_dev && out && count > 0, "idiff_latent_mean: bad arguments");
   IDIFF_CHECK_CUDA(launch_pdl(latent_mean_kernel, dim3(grid_for(n, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), xs_dev, count, out, n));
+  IDIFF_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int idiff_conv_in_select(const float* x, const void* w0, const float* b0, const void* w1, const float* b1,
+                                    const int* flags, void* out, int batch, int h, int w, int cout, void* stream) {
+  IDIFF_REQUIRE(x && w0 && b0 && w1 && b1 && flags && out, "idiff_conv_in_select: null pointer argument");
+  IDIFF_REQUIRE(batch > 0 && h > 0 && w > 0 && cout > 0 && cout % 2 == 0 && cout <= 1024,
+                "idiff_conv_in_select: bad shape (batch %d, %dx%d, cout %d)", batch, h, w, cout);
+  const size_t smem = sizeof(float4) * (CONV_IN_ROWS + 2) * (w + 2);
+  IDIFF_REQUIRE(smem <= 48 * 1024, "idiff_conv_in_select: width %d too large", w);
+  dim3 grid((h + CONV_IN_ROWS - 1) / CONV_IN_ROWS, batch);
+  IDIFF_CHECK_CUDA(launch_pdl(conv_in_select_kernel, grid, dim3(cout / 2), smem, reinterpret_cast<cudaStream_t>(stream), x,
+                              reinterpret_cast<const h16*>(w0), b0, reinterpret_cast<const h16*>(w1), b1, flags,
+                              reinterpret_cast<uint32_t*>(out), h, w, cout));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

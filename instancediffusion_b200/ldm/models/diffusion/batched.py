@@ -32,8 +32,9 @@ from ._plms_common import PLMSBase, Trajectory
 class Request:
     """One sampling request.  `input`: the dict `PLMSSampler.sample` takes, or the list [global, inst_1 .. inst_n]
     of `PLMSSamplerInst.sample`; `shape`: (B, 4, H, W) of its latent (may be omitted when input x is given);
-    `mis`: the Multi-instance fraction (list inputs only).  `S`, if given, must equal the call's step count.
-    `mask` / `x0` (inpainting) are not supported and raise."""
+    `mis`: the Multi-instance fraction (list inputs only).  `S`: the request's step count; `sample_requests` takes it
+    from the call (S, if given, must equal it), `SamplingEngine` requires it.  `mask` / `x0` (inpainting) are not
+    supported and raise."""
     input: Union[dict, List[dict]]
     uc: Optional[torch.Tensor] = None
     guidance_scale: float = 1.0
@@ -169,11 +170,14 @@ class _State:
         self.trajs = self.trajs[:1]
 
 
-def _evaluate(model, states: List[_State], slots: List[Tuple[int, int]], max_batch: int, scales, restored, null_inputs):
-    """One UNet evaluation of the given trajectories, in forward chunks: {(request, trajectory): (e_c, e_u|None)}."""
-    plans = [s.plan for s in states]
+def _evaluate(model, states: List[_State], chunks: Sequence[Tuple[List[Tuple[int, int]], Optional[int]]], scales,
+              restored, null_inputs, per_image_conv: bool = False):
+    """One UNet evaluation of the trajectories of `chunks`, one forward per (chunk, padded size): {(request, trajectory):
+    (e_c, e_u|None)}.  A chunk with a padded size is filled up to it with copies of its last input (same context and
+    grounding, so its hoisted tensors come from the caches) with a zero latent, fuser scale 0 and the model's own
+    conv; their outputs are dropped.  per_image_conv: see UNetModel.forward_batched."""
     out = {}
-    for chunk in plan_chunks(slots, plans, max_batch):
+    for chunk, padded in chunks:
         inputs, sc, rs = [], [], []
         for r, k in chunk:
             st = states[r]
@@ -185,7 +189,14 @@ def _evaluate(model, states: List[_State], slots: List[Tuple[int, int]], max_bat
             n = 2 if st.plan.cfg else 1
             sc += [scales[r]] * n
             rs += [restored[r]] * n
-        outs = model.forward_batched(inputs, scales=sc, restored=rs)
+        if padded is not None:
+            last = inputs[-1]
+            pad = dict(last, x=torch.zeros_like(last["x"]))
+            n_pad = (padded - sum(i["x"].shape[0] for i in inputs)) // last["x"].shape[0]
+            inputs += [pad] * n_pad
+            sc += [0.0] * n_pad
+            rs += [False] * n_pad
+        outs = model.forward_batched(inputs, scales=sc, restored=rs, per_image_conv=per_image_conv)
         j = 0
         for r, k in chunk:
             if states[r].plan.cfg:
@@ -283,13 +294,16 @@ def _run(model, base, states, time_range, total, max_batch, entry_scale, entry_r
             for tr in st.trajs:
                 tr.input["timesteps"] = ts
         slots = [(r, k) for r, st in enumerate(states) for k in range(len(st.trajs))]
-        evals = _evaluate(model, states, slots, max_batch, scales, restored, null_inputs)
+        plans = [st.plan for st in states]
+        evals = _evaluate(model, states, [(c, None) for c in plan_chunks(slots, plans, max_batch)], scales, restored,
+                          null_inputs)
         pending = {}
         for r, st in enumerate(states):
             pending[r] = base._step_predict(st.trajs, [evals[(r, k)] for k in range(len(st.trajs))], steps[r], index,
                                             st.gs)
         again = [(r, k) for r, k in slots if pending[r] is not None]
         if again:  # first step of a trajectory: the corrector's evaluation at t_next
-            evals.update(_evaluate(model, states, again, max_batch, scales, restored, null_inputs))
+            evals.update(_evaluate(model, states, [(c, None) for c in plan_chunks(again, plans, max_batch)], scales,
+                                   restored, null_inputs))
         for r, st in enumerate(states):
             base._step_finish(st.trajs, [evals[(r, k)] for k in range(len(st.trajs))], pending[r], index, st.gs)

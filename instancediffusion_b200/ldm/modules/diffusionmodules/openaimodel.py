@@ -24,7 +24,7 @@ import torch
 import torch.nn as nn
 
 from .... import ops
-from ....packing import pack_conv1x1, pack_conv3x3
+from ....packing import pack_conv1x1, pack_conv3x3, pack_conv3x3_taps
 from ...util import instantiate_from_config
 from .._base import half, PackedModule, f32, nchw_to_nhwc16, nhwc16_to_nchw, w16
 from ..attention import SpatialTransformer, attention_mask_words
@@ -225,6 +225,8 @@ class UNetModel(PackedModule):
     # (one per combination of inputs in a batched forward); a cache that reaches its bound is cleared
     hoist_cache_entries = 64
     cat_cache_entries = 6
+    # memory pool token (torch.cuda.graph_pool_handle()) that new graph captures share; None: a private pool each
+    graph_pool = None
 
     def __init__(self, image_size, in_channels, model_channels, out_channels, num_res_blocks,
                  attention_resolutions, dropout=0, channel_mult=(1, 2, 4, 8), conv_resample=True, dims=2,
@@ -366,7 +368,8 @@ class UNetModel(PackedModule):
         # unless different SD weights than last time are supplied.
         if getattr(self, "_sd_conv_src", None) is not sd_weights:
             self._sd_conv_src = sd_weights
-            self._in_packs.pop(True, None)
+            self._in_packs.pop((True, False), None)
+            self._in_packs.pop((True, True), None)
             for k in [k for k in self._graphs if k[-1]]:
                 del self._graphs[k]
 
@@ -379,13 +382,14 @@ class UNetModel(PackedModule):
             self.input_blocks[0][0] = conv.to(self.input_blocks[0][0].weight.device)
             self._first_conv_restored = False
 
-    def _in_conv_pack(self, restored: Optional[bool] = None):
+    def _in_conv_pack(self, restored: Optional[bool] = None, taps: bool = False):
         """Packed input conv of the model's current first-conv state, or (restored=True / False) of the SD1.5 /
         the model's own conv whatever the current state is.  The SD weights are the ones last given to
-        set_sd_first_conv, else load_sd_first_conv()."""
+        set_sd_first_conv, else load_sd_first_conv().  taps: in the layout of ops.conv_in_select instead of the
+        conv GEMM's."""
         cur = bool(getattr(self, "_first_conv_restored", False))
         key = cur if restored is None else bool(restored)
-        hit = self._in_packs.get(key)
+        hit = self._in_packs.get((key, taps))
         if hit is None:
             conv0 = self.input_blocks[0][0]
             if key == cur:
@@ -396,9 +400,18 @@ class UNetModel(PackedModule):
                     sd = self.load_sd_first_conv()
                 w, b = sd["weight"].to(conv0.weight.device), sd["bias"].to(conv0.weight.device)
             with torch.no_grad():
-                hit = (_pack_conv3x3_padded(w, 64), f32(b))
-            self._in_packs[key] = hit
+                hit = (pack_conv3x3_taps(w.detach().to(half())) if taps else _pack_conv3x3_padded(w, 64), f32(b))
+            self._in_packs[(key, taps)] = hit
         return hit
+
+    def _in_conv_taps(self):
+        """((w0, b0, w1, b1) of ops.conv_in_select: the model's own input conv and the SD1.5 one, whether the SD1.5
+        weights exist).  Without them both sets are the model's own conv, and no image may select the second."""
+        own = self._in_conv_pack(False, taps=True)
+        try:
+            return own + self._in_conv_pack(True, taps=True), True
+        except FileNotFoundError:
+            return own + own, False
 
     def _drop_derived(self):
         """Everything computed from the weights: packed first conv, captured graphs, hoisted text K/V and
@@ -500,8 +513,7 @@ class UNetModel(PackedModule):
                    str(gi["boxes"].device))
         else:
             gi = grounding_input
-            key = tuple(self._tkey(gi[k]) for k in ("boxes", "masks", "positive_embeddings", "scribbles",
-                                                   "polygons", "segs", "points", "att_masks") if gi.get(k) is not None)
+            key = self._obj_key(gi)
         hit = self._obj_cache.get(key)
         if hit is not None:
             return hit[1]
@@ -516,6 +528,30 @@ class UNetModel(PackedModule):
         val = (kvs, Bo, n_obj, mask)
         self._obj_cache[key] = (gi, val)
         return val
+
+    def _obj_key(self, gi: dict):
+        return tuple(self._tkey(gi[k]) for k in ("boxes", "masks", "positive_embeddings", "scribbles", "polygons",
+                                                "segs", "points", "att_masks") if gi.get(k) is not None)
+
+    def drop_hoisted(self, inputs: List[dict], keep: List[dict] = ()):
+        """Drop the hoisted tensors of `inputs` (text K/V of their context, object K/V of their grounding input) and
+        every batch concatenation that holds one of them, except those that the inputs in `keep` share.  What a
+        server calls when a request finishes."""
+        def keys(ins):
+            return ({self._tkey(i["context"]) for i in ins},
+                    {self._obj_key(i["grounding_input"]) for i in ins if i.get("grounding_input") is not None})
+        ctx_keys, obj_keys = keys(inputs)
+        kept_ctx, kept_obj = keys(keep)
+        gone = [self._ctx_cache.pop(k) for k in ctx_keys - kept_ctx if k in self._ctx_cache]
+        gone_obj = [self._obj_cache.pop(k) for k in obj_keys - kept_obj if k in self._obj_cache]
+        ids = {id(v[1]) for v in gone} | {id(v[1][0]) for v in gone_obj} | {id(v[1][3]) for v in gone_obj if v[1][3] is not None}
+        for k in [k for k in self._cat_cache if ids & set(k[2] + k[3] + k[4])]:
+            del self._cat_cache[k]
+
+    def trim_concats(self, keep: int):
+        """Keep only the `keep` most recently used batch concatenations of the hoisted tensors."""
+        for k in list(self._cat_cache)[:max(len(self._cat_cache) - int(keep), 0)]:
+            del self._cat_cache[k]
 
     def clear_hoisted(self):
         """Drop the per-sample hoisted tensors (text K/V, UniFusion tokens / object K/V, their concatenations);
@@ -545,11 +581,12 @@ class UNetModel(PackedModule):
 
     def _core(self, x: torch.Tensor, t: torch.Tensor, ctx_kv_all: torch.Tensor, M: int,
               obj_kvs: Optional[List[torch.Tensor]], n_obj: int, mask=None, fuser_scale=None,
-              n_restored: Optional[int] = None) -> torch.Tensor:
+              n_restored=None) -> torch.Tensor:
         """x fp32 (B,4,H,W), t fp32 (B,), ctx_kv_all fp16 [B*M, sumKV], obj_kvs per-fuser [B*n_obj, 2C]
         (or None on alpha=0 steps) -> eps fp32 (B,4,H,W).  fuser_scale: None (each fuser's `.scale`), a float or
-        an fp32 [B] tensor of per-image scales.  n_restored: None (the model's first-conv state for every image) or
-        the number of trailing images that take the SD1.5 input conv, the others the model's own."""
+        an fp32 [B] tensor of per-image scales.  n_restored: None (the model's first-conv state for every image),
+        the number of trailing images that take the SD1.5 input conv, the others the model's own, or an int32 [B]
+        device tensor of per-image flags (1: the SD1.5 conv) for ops.conv_in_select."""
         p = self.pk()
         B, _, H, W = x.shape
         # time embedding (openaimodel.py:497-498) ; SiLU of emb_layers[0] folded into the last epilogue
@@ -590,11 +627,14 @@ class UNetModel(PackedModule):
                     raise TypeError(f"unexpected layer {type(layer)}")
             return h, hh, ww
 
-        x16 = ops.nchw_f32_to_nhwc_f16(x, 64)
-        if n_restored is None or n_restored in (0, B):
+        if isinstance(n_restored, torch.Tensor):
+            h = ops.conv_in_select(x, *self._in_conv_taps()[0], n_restored)
+        elif n_restored is None or n_restored in (0, B):
+            x16 = ops.nchw_f32_to_nhwc_f16(x, 64)
             w_in, b_in = self._in_conv_pack(None if n_restored is None else n_restored == B)
             h = ops.gemm(x16, w_in, b_in, conv=(B, H, W, 64))
         else:  # one conv GEMM per first-conv state, each on its contiguous range of images
+            x16 = ops.nchw_f32_to_nhwc_f16(x, 64)
             h = torch.empty((B * H * W, self.model_channels), dtype=half(), device=x.device)
             for b0, nb, restored in ((0, B - n_restored, False), (B - n_restored, n_restored, True)):
                 w_in, b_in = self._in_conv_pack(restored)
@@ -657,8 +697,9 @@ class UNetModel(PackedModule):
         # the hoisted tensors above are cached objects: their identities (and the batch sizes) name the combination
         key = (active, tuple(bs), tuple(id(c) for c in ctxs), tuple(id(k) for k, _ in okv_lists),
                tuple(id(m) for m, _ in masks))
-        hit = self._cat_cache.get(key)
+        hit = self._cat_cache.pop(key, None)
         if hit is not None:
+            self._cat_cache[key] = hit  # most recently used last (trim_concats)
             _, ctx, okv, mask = hit
             return x, t, ctx, M, okv, n_obj, mask
         ctx = ctxs[0] if len(inputs) == 1 else torch.cat(ctxs, 0)
@@ -693,14 +734,17 @@ class UNetModel(PackedModule):
 
     @torch.no_grad()
     def forward_batched(self, inputs: List[dict], *, scales: Optional[List[float]] = None,
-                        restored: Optional[List[bool]] = None) -> List[torch.Tensor]:
+                        restored: Optional[List[bool]] = None, per_image_conv: bool = False) -> List[torch.Tensor]:
         """Run several independent forwards as one batch; returns one eps tensor per input.
 
         scales: one fuser scale per input -- what set_alpha_scale would set for a forward of that input alone --
         instead of the fusers' own `.scale`.  Equal scales run the scalar-gate path (all 0: the fusers are skipped);
         mixed scales run the fusers on every image with the gates tanh(alpha) * scale of each image.
         restored: per input, True = the SD1.5 input conv that restore_first_conv_from_SD swaps in, False = the
-        model's own; the model's conv is not swapped.  Default: the model's current first-conv state."""
+        model's own; the model's conv is not swapped.  Default: the model's current first-conv state.
+        per_image_conv: choose each image's input conv on the device (ops.conv_in_select) from a per-image flag that,
+        like the per-image scales, is a static input of the captured graph.  The count of SD1.5-conv images then
+        stays out of the graph key, and the images keep their order."""
         if getattr(self, "_storage_epoch", None) != ops.STORAGE_EPOCH:  # storage type switched: derived tensors are stale
             self._drop_derived()
             self._storage_epoch = ops.STORAGE_EPOCH
@@ -709,7 +753,15 @@ class UNetModel(PackedModule):
             if arg is not None and len(arg) != n:
                 raise ValueError(f"forward_batched: {len(arg)} {name} for {n} inputs")
         sizes = [inp["x"].shape[0] for inp in inputs]
-        if restored is None:
+        if per_image_conv:
+            order = list(range(n))
+            cur = bool(getattr(self, "_first_conv_restored", False))
+            flags = [bool(restored[i]) if restored is not None else cur for i in range(n)]
+            if any(flags):
+                self._in_conv_pack(True, taps=True)  # raises when no SD1.5 conv weights exist
+            rows_in = torch.tensor([int(f) for f, b in zip(flags, sizes) for _ in range(b)], dtype=torch.int32)
+            n_restored = rows_in.pin_memory().to(inputs[0]["x"].device, non_blocking=True)
+        elif restored is None:
             order = list(range(n))
             n_restored = sum(sizes) if getattr(self, "_first_conv_restored", False) else 0
         else:  # images of the SD1.5 conv last: each input conv is one GEMM over a contiguous range of images
@@ -747,13 +799,18 @@ class UNetModel(PackedModule):
                            for st in self._transformers() for blk in st.transformer_blocks)
         if n_restored is None:
             n_restored = x.shape[0] if getattr(self, "_first_conv_restored", False) else 0
-        # (set_sd_first_conv drops the graphs whose last key entry, the count of SD-conv images, is non-zero)
-        key = (tuple(x.shape), M, scales, n_obj, mask is not None, n_restored)
+        # per-image conv flags are a static input buffer; the graph points at both packed convs (or twice at the
+        # model's own while no SD1.5 weights exist)
+        conv = n_restored
+        if isinstance(n_restored, torch.Tensor):
+            conv = "per-image" if self._in_conv_taps()[1] else "per-image, own conv only"
+        # (set_sd_first_conv drops the graphs whose last key entry, the count of SD-conv images, is truthy)
+        key = (tuple(x.shape), M, scales, n_obj, mask is not None, conv)
         g = self._graphs.get(key)
         if g is None:
             g = _CoreGraph(self, x, t, ctx, M, okv, n_obj, mask, fuser_scale, n_restored)
             self._graphs[key] = g
-        return g.replay(x, t, ctx, okv, mask, fuser_scale)
+        return g.replay(x, t, ctx, okv, mask, fuser_scale, n_restored)
 
     def forward_single_input(self, input):
         return self.forward_batched([input])[0]
@@ -774,6 +831,7 @@ class _CoreGraph:
         self.mask = (mask[0].clone(), mask[1].clone()) if mask is not None else None
         # per-image fuser scales: a static input like x and t (a float or None is part of the graph key)
         self.scale = fuser_scale.clone() if isinstance(fuser_scale, torch.Tensor) else fuser_scale
+        self.conv = n_restored.clone() if isinstance(n_restored, torch.Tensor) else n_restored
         model.pk()  # make sure packing (allocations + host work) happens outside capture
         for st in model._transformers():
             st.pk()
@@ -789,17 +847,19 @@ class _CoreGraph:
             s = torch.cuda.Stream()
             s.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(s):
-                model._core(self.x, self.t, self.ctx, M, self.okv, n_obj, self.mask, self.scale, n_restored)
+                model._core(self.x, self.t, self.ctx, M, self.okv, n_obj, self.mask, self.scale, self.conv)
             torch.cuda.current_stream().wait_stream(s)
             self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
-                self.out = model._core(self.x, self.t, self.ctx, M, self.okv, n_obj, self.mask, self.scale, n_restored)
+            with torch.cuda.graph(self.graph, pool=model.graph_pool):
+                self.out = model._core(self.x, self.t, self.ctx, M, self.okv, n_obj, self.mask, self.scale, self.conv)
 
-    def replay(self, x, t, ctx, okv, mask=None, fuser_scale=None):
+    def replay(self, x, t, ctx, okv, mask=None, fuser_scale=None, n_restored=None):
         self.x.copy_(x)
         self.t.copy_(t)
         if isinstance(self.scale, torch.Tensor):
             self.scale.copy_(fuser_scale)
+        if isinstance(self.conv, torch.Tensor):
+            self.conv.copy_(n_restored)
         # step-invariant inputs: the static buffers already hold them when the very same (immutable, cached)
         # tensor objects come back -- every step of a sampling run after the first
         last = getattr(self, "_last", (None, None, None))

@@ -474,6 +474,34 @@ def latent_mean(xs, out: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def conv_in_select(x: torch.Tensor, w0: torch.Tensor, b0: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor,
+                   flags: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The UNet input conv with a weight set per image: x fp32 (B, 4, H, W); w0 / w1 16-bit [36, Cout]
+    (packing.pack_conv3x3_taps); b0 / b1 fp32 [Cout]; flags int32 (B,) on the device, 0 -> (w0, b0), else
+    (w1, b1).  Returns 16-bit NHWC [B*H*W, Cout], the activation the first ResBlock reads."""
+    lib = _lib.load()
+    _req(x, torch.float32, "x")
+    _req(flags, torch.int32, "flags")
+    B, Cc, H, W = x.shape
+    cout = w0.shape[1]
+    for name, w, b in (("w0", w0, b0), ("w1", w1, b1)):
+        _req(w, HALF, name)
+        _req(b, torch.float32, name.replace("w", "b"))
+        if tuple(w.shape) != (36, cout) or not w.is_contiguous() or b.numel() != cout:
+            raise _lib.IdiffError(f"conv_in_select: {name} {tuple(w.shape)} / bias {tuple(b.shape)} are not [36, {cout}] / [{cout}]")
+    if Cc != 4 or flags.numel() != B or not flags.is_contiguous():
+        raise _lib.IdiffError(f"conv_in_select: x {tuple(x.shape)} needs 4 channels and flags {B} entries")
+    x = x.contiguous()
+    if out is None:
+        out = torch.empty((B * H * W, cout), dtype=HALF, device=x.device)
+    _req(out, HALF, "out")
+    check(_launch("conv_in_select", 2.0 * B * H * W * cout * 36, 4.0 * x.numel() + 2.0 * out.numel(),
+                  lambda: lib.idiff_conv_in_select(x.data_ptr(), w0.data_ptr(), b0.data_ptr(), w1.data_ptr(), b1.data_ptr(),
+                                                   flags.data_ptr(), out.data_ptr(), B, H, W, cout, _stream())),
+          "idiff_conv_in_select")
+    return out
+
+
 def silu(x: torch.Tensor) -> torch.Tensor:
     lib = _lib.load()
     _req(x, HALF, "x")

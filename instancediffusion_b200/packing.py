@@ -17,6 +17,14 @@ def pack_conv3x3(w: torch.Tensor) -> torch.Tensor:
     return w.permute(0, 2, 3, 1).reshape(cout, 9 * cin).contiguous()
 
 
+def pack_conv3x3_taps(w: torch.Tensor) -> torch.Tensor:
+    """(Cout, Cin, 3, 3) -> (9*Cin, Cout) with row k = (ky*3 + kx)*Cin + c: the layout of
+    idiff_conv_in_select, whose threads each read a pair of output channels."""
+    cout, cin, kh, kw = w.shape
+    assert kh == 3 and kw == 3
+    return w.permute(2, 3, 1, 0).reshape(9 * cin, cout).contiguous()
+
+
 def pack_conv1x1(w: torch.Tensor) -> torch.Tensor:
     """(Cout, Cin, 1, 1) -> (Cout, Cin)."""
     return w.reshape(w.shape[0], w.shape[1]).contiguous()
