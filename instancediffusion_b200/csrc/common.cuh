@@ -158,6 +158,25 @@ IDIFF_DEVICE void tma_store_4d(const CUtensorMap* m, const void* src, int c0, in
 IDIFF_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
 // all bulk groups of this thread have finished READING shared memory (buffers reusable)
 IDIFF_DEVICE void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }
+// all bulk groups of this thread have completed (their global writes are done)
+IDIFF_DEVICE void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory"); }
+
+// ----------------------------------------------------------------------------------
+// ldmatrix / stmatrix: four 8x8 16-bit matrices between shared memory and the mma fragment layout
+// (thread t holds row t/4, columns 2(t%4) and 2(t%4)+1 of matrix i in r[i]); lanes 8i..8i+7 give the
+// row addresses (16 B each) of matrix i.
+// ----------------------------------------------------------------------------------
+IDIFF_DEVICE void ldmatrix_x4(uint32_t (&r)[4], uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];\n"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(saddr)
+               : "memory");
+}
+IDIFF_DEVICE void stmatrix_x4(uint32_t saddr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"(saddr), "r"(r[0]),
+               "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
 
 // ----------------------------------------------------------------------------------
 // numerics

@@ -13,11 +13,18 @@
 //     the owner adds them in a fixed order -> bit-reproducible.
 //   * BN in {128, 160, 192, 256} chosen per N (320 = 2 x 160, 960 = 5 x 192, 1280 = 5 x 256 ...):
 //     no padded columns, half the A-tile traffic of 128-wide tiles.
-//   * warp roles (384 threads = 3 warpgroups): warpgroup 0 is the TMA producer (one thread; the group
-//     gives its registers to the consumers with setmaxnreg), warpgroups 1 and 2 are consumers that
-//     own 64 rows of the tile each: wgmma m64nBNk16 from the 128B-swizzled operand ring into register
-//     accumulators, then the fused epilogue straight from the accumulator fragments.  The producer
-//     runs ahead across segments, so the next tile's operands land while the consumers store.
+//   * warp roles (384 threads = 3 warpgroups): warpgroup 0 holds the TMA producer (warp 0, one thread)
+//     and the epilogue store warp (warp 1, one thread); the group gives its registers to the consumers
+//     with setmaxnreg.  Warpgroups 1 and 2 are consumers that own 64 rows of the tile each: wgmma
+//     m64nBNk16 from the 128B-swizzled operand ring into register accumulators, then the fused epilogue.
+//     The producer runs ahead across segments, so the next tile's operands land during the epilogue.
+//   * staged epilogue (16-bit outputs): one tile-sized buffer in shared memory, in 32-column slabs of
+//     128 rows x 64 B (64B swizzle).  The store warp TMA-loads the tile's residual into it while the
+//     consumers run the mainloop; the consumers read it with ldmatrix in accumulator-fragment order,
+//     write the packed result back in place with stmatrix and go straight on to the next tile's
+//     mainloop; the store warp writes the buffer out with TMA stores (rows past M / past the conv
+//     image, columns past N clipped by the tensor map) and reloads it for the next tile once the
+//     stores have read it.  Only the final conv's fp32 NCHW output is stored from the fragments.
 // conv3x3 gathers the A tile tap by tap with a 4-D TMA box over the NHWC activation; out-of-image taps
 // are zero-filled by the TMA unit (no im2col buffer, no halo copy).
 #include "../../include/idiff_b200.h"
@@ -62,17 +69,30 @@ struct Params {
   float ln_eps;
 };
 
-template <int BN>
+constexpr int MODE_PLAIN = 0;  // bias / row-add, optional SiLU / GELU, optional gate*x + residual, fp16 out
+constexpr int MODE_GEGLU = 1;  // (value + b) * gelu(gate + b), fp16 out with N/2 columns
+constexpr int MODE_NCHW = 2;   // fp32 (B, N, HW) output (the final conv -> eps)
+constexpr int MODE_GATED = 3;  // bias, gate * gate_b[batch entry] * x + residual, fp16 out (per-image fuser scales)
+
+constexpr int EPI_SLAB_COLS = 32;                        // columns of one epilogue slab / TMA box (64 B rows)
+constexpr int EPI_SLAB_BYTES = BM * EPI_SLAB_COLS * 2;   // 8 KB
+
+template <int BN, int MODE>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  static constexpr int BAR_BYTES = 256;          // 2 * STAGES mbarriers
+  // epilogue buffer: the 128 x EW output tile (GEGLU: BN/2 columns; none for the fp32 NCHW output)
+  static constexpr int EW = MODE == MODE_NCHW ? 0 : MODE == MODE_GEGLU ? BN / 2 : BN;
+  static constexpr int EPI_BYTES = BM * EW * 2;
+  static constexpr int BAR_BYTES = 256;          // 2 * STAGES + 2 mbarriers
   static constexpr int FIXED = 1024 + BAR_BYTES;  // + slack to align the ring to 1024 B (SWIZZLE_128B)
-  static constexpr int STAGES_FIT = (227 * 1024 - FIXED) / STAGE_BYTES;
+  static constexpr int STAGES_FIT = (227 * 1024 - FIXED - EPI_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 6 ? 6 : STAGES_FIT;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + FIXED;
   static constexpr int ACC = BN / 2;  // fp32 accumulator registers per consumer thread (64 x BN per warpgroup)
   static_assert(STAGES >= 3, "operand ring too shallow");
+  static_assert(EW % EPI_SLAB_COLS == 0, "epilogue slabs must tile the output columns exactly");
+  static_assert(STAGE_BYTES % 1024 == 0, "the epilogue buffer after the ring must stay 1024 B aligned");
 };
 
 struct Seg {
@@ -123,23 +143,29 @@ IDIFF_DEVICE void st_release_gpu(int* p, int v) {
 }
 IDIFF_DEVICE float2 ld_pair(const h16* p) { return unpack_half2(*reinterpret_cast<const uint32_t*>(p)); }
 
-constexpr int MODE_PLAIN = 0;  // bias / row-add, optional SiLU / GELU, optional gate*x + residual, fp16 out
-constexpr int MODE_GEGLU = 1;  // (value + b) * gelu(gate + b), fp16 out with N/2 columns
-constexpr int MODE_NCHW = 2;   // fp32 (B, N, HW) output (the final conv -> eps)
-constexpr int MODE_GATED = 3;  // bias, gate * gate_b[batch entry] * x + residual, fp16 out (per-image fuser scales)
+// Byte offset in the epilogue buffer of the 16 B chunk holding tile row `row`, columns [8 jj, 8 jj + 8):
+// 32-column slabs of 128 rows x 64 B, each row's four chunks permuted as the TMA unit's 64B swizzle does
+// (chunk ^= (row / 2) % 4), so the 8 rows of one ldmatrix / stmatrix phase hit 8 different 16 B bank groups.
+IDIFF_DEVICE uint32_t epi_offset(int row, int jj) {
+  return (uint32_t)((jj >> 2) * EPI_SLAB_BYTES + row * 64 + (((jj & 3) ^ ((row >> 1) & 3)) << 4));
+}
 
 template <int BN, int MODE>
 __global__ void __launch_bounds__(THREADS, 1)
-gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
-  using C = Cfg<BN>;
+gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+             const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR, const Params p) {
+  using C = Cfg<BN, MODE>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * C::STAGE_BYTES);
+  uint8_t* sE = smem + STAGES * C::STAGE_BYTES;  // epilogue buffer (C::EPI_BYTES)
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sE + C::EPI_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* epi_ready = empty_bar + STAGES;  // the tile's residual has landed in sE (or: sE is free, no residual)
+  uint64_t* epi_full = epi_ready + 1;        // the consumers have staged the tile's output in sE
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -148,10 +174,16 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (C::EW > 0) {
+      tma_prefetch_desc(&tmO);
+      if (p.residual) tma_prefetch_desc(&tmR);
+    }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], CONSUMER_WARPS);  // one arrival per consumer warp
     }
+    mbar_init(epi_ready, 1);
+    mbar_init(epi_full, 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -162,6 +194,13 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       unsigned long long t;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
       p.trace[(long)blockIdx.x * 16 + slot] = t;
+    }
+  };
+  // a phase of the CTA's first and of its last epilogue tile: slot (kept once written) and slot + 3
+  auto stamp_tile = [&](int slot) {
+    if (p.trace) {
+      if (p.trace[(long)blockIdx.x * 16 + slot] == 0) stamp(slot);
+      stamp(slot + 3);
     }
   };
   if (threadIdx.x == 0) {
@@ -226,6 +265,42 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           }
         }
       }
+    } else if (C::EW > 0 && warp == 1 && lane == 0) {
+      // ===================== epilogue store warp: residual in, result out =====================
+      // Per owner segment (the ones that run an epilogue): fill sE with the tile's residual (or just
+      // release it to the consumers), wait until they have staged the result there, store it, and wait
+      // until the stores have read sE before the next tile's residual may overwrite it.
+      WorkIter it(p, cta);
+      Seg sg;
+      uint32_t ep = 0;
+      const int n_out = MODE == MODE_GEGLU ? p.N / 2 : p.N;
+      while (it.next(sg)) {
+        if (sg.kb0 != 0) continue;
+        int n0, m0, b0, h0, w0;
+        tile_origin(sg.tile, n0, m0, b0, h0, w0);
+        const int oc0 = MODE == MODE_GEGLU ? (sg.tile % p.n_tiles) * (BN / 2) : n0;
+        const int rem = (n_out - oc0 + EPI_SLAB_COLS - 1) / EPI_SLAB_COLS;  // slabs not wholly past N
+        const int slabs = rem < C::EW / EPI_SLAB_COLS ? rem : C::EW / EPI_SLAB_COLS;
+        if (p.residual) {
+          mbar_expect_tx(epi_ready, slabs * EPI_SLAB_BYTES);  // clipped box elements count (zero-filled)
+          for (int q = 0; q < slabs; ++q) {
+            if (p.conv) tma_load_4d(sE + q * EPI_SLAB_BYTES, &tmR, epi_ready, oc0 + q * EPI_SLAB_COLS, w0, h0, b0);
+            else tma_load_2d(sE + q * EPI_SLAB_BYTES, &tmR, epi_ready, oc0 + q * EPI_SLAB_COLS, m0);
+          }
+        } else {
+          mbar_arrive(epi_ready);
+        }
+        mbar_wait(epi_full, ep);
+        ep ^= 1;
+        for (int q = 0; q < slabs; ++q) {
+          if (p.conv) tma_store_4d(&tmO, sE + q * EPI_SLAB_BYTES, oc0 + q * EPI_SLAB_COLS, w0, h0, b0);
+          else tma_store_2d(&tmO, sE + q * EPI_SLAB_BYTES, oc0 + q * EPI_SLAB_COLS, m0);
+        }
+        tma_store_commit();
+        stamp_tile(3);
+        tma_store_wait_read();
+      }
+      tma_store_wait_all();
     }
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
@@ -252,6 +327,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     WorkIter it(p, cta);
     Seg sg;
     uint32_t s = 0, ph = 0;
+    uint32_t ep = 0;  // epilogue buffer phase
     while (it.next(sg)) {
       int n0, m0, b0, h0, w0;
       tile_origin(sg.tile, n0, m0, b0, h0, w0);
@@ -278,6 +354,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
       const bool owner = sg.kb0 == 0;
+      if (owner && ct == 0) stamp_tile(1);
       const bool complete = owner && sg.kb1 == p.KB;
       const bool fixup = owner && !complete;  // this CTA holds the tile's first k-blocks, others the rest
       const long fstride = (long)BM * BN / 4;  // float4s of one CTA's partial tile
@@ -323,7 +400,7 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           for (int f = f0; f <= f1; ++f) st_release_gpu(p.sflags + f * CONSUMER_WARPS + ew, 0);
       }
 
-      // ---- fused epilogue, straight from the fragments: rows rl0 / rl0 + 8, column pairs 8j + 2 t4 ----
+      // ---- fused epilogue: rows rl0 / rl0 + 8, column pairs 8j + 2 t4 ----
       long orow[2];
       bool rok[2];
       int bidx[2], pix[2];
@@ -379,13 +456,13 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         for (int hh = 0; hh < 2; ++hh)
           if (rok[hh]) gate_r[hh] = gate * __ldg(p.gate_b + bidx[hh]);
       }
-#pragma unroll
-      for (int j = 0; j < NJO; ++j) {
+      // column vectors of the 8-column group j at this thread's column pair (zero for columns past N)
+      auto col_vecs = [&](int j, float2& bv, float2& bg, float2& sv, float2& sgt) {
         const int c = 8 * j + 2 * t4;  // tile column of the pair (GEGLU: value column; its gate is BN/2 further on)
         const int oc = out_col_base + c;
-        if (oc >= n_out_total) continue;  // 16-bit outputs have N % 8 == 0: a pair is wholly inside or outside
+        bv = bg = sv = sgt = make_float2(0.f, 0.f);
+        if (oc >= n_out_total) return;  // 16-bit outputs have N % 8 == 0: a pair is wholly inside or outside
         const bool hi = !nchw || oc + 1 < n_out_total;  // fp32 NCHW output may have an odd N (the final conv: 3 or 4)
-        float2 bv = make_float2(0.f, 0.f), bg = bv, sv = bv, sgt = bv;
         if (p.bias) {
           if (nchw) bv = make_float2(__ldg(p.bias + n0 + c), hi ? __ldg(p.bias + n0 + c + 1) : 0.f);
           else bv = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c));
@@ -395,60 +472,109 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           sv = __ldg(reinterpret_cast<const float2*>(p.ln_s + n0 + c));
           if (geglu) sgt = __ldg(reinterpret_cast<const float2*>(p.ln_s + n0 + BN / 2 + c));
         }
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          if (!rok[hh]) continue;
-          float x0 = acc[4 * j + 2 * hh], x1 = acc[4 * j + 2 * hh + 1];
+      };
+      // bias or LayerNorm fold, then GEGLU, or row-add and SiLU / GELU, of the pair (j, row half hh)
+      auto act_pair = [&](int j, int hh, const float2& bv, const float2& bg, const float2& sv, const float2& sgt,
+                          float& x0, float& x1) {
+        x0 = acc[4 * j + 2 * hh];
+        x1 = acc[4 * j + 2 * hh + 1];
+        if (lni) {
+          x0 = fmaf(ln_rstd[hh], x0, fmaf(ln_nmean[hh], sv.x, bv.x));
+          x1 = fmaf(ln_rstd[hh], x1, fmaf(ln_nmean[hh], sv.y, bv.y));
+        } else {
+          x0 += bv.x;
+          x1 += bv.y;
+        }
+        if (geglu) {
+          float g0 = acc[4 * (j + NJ / 2) + 2 * hh], g1 = acc[4 * (j + NJ / 2) + 2 * hh + 1];
           if (lni) {
-            x0 = fmaf(ln_rstd[hh], x0, fmaf(ln_nmean[hh], sv.x, bv.x));
-            x1 = fmaf(ln_rstd[hh], x1, fmaf(ln_nmean[hh], sv.y, bv.y));
+            g0 = fmaf(ln_rstd[hh], g0, fmaf(ln_nmean[hh], sgt.x, bg.x));
+            g1 = fmaf(ln_rstd[hh], g1, fmaf(ln_nmean[hh], sgt.y, bg.y));
           } else {
-            x0 += bv.x;
-            x1 += bv.y;
+            g0 += bg.x;
+            g1 += bg.y;
           }
-          if (geglu) {
-            float g0 = acc[4 * (j + NJ / 2) + 2 * hh], g1 = acc[4 * (j + NJ / 2) + 2 * hh + 1];
-            if (lni) {
-              g0 = fmaf(ln_rstd[hh], g0, fmaf(ln_nmean[hh], sgt.x, bg.x));
-              g1 = fmaf(ln_rstd[hh], g1, fmaf(ln_nmean[hh], sgt.y, bg.y));
-            } else {
-              g0 += bg.x;
-              g1 += bg.y;
-            }
-            x0 *= gelu_erf_f(g0);
-            x1 *= gelu_erf_f(g1);
-          } else {
-            if (!gated && p.rowadd) {
-              const float2 f = ld_pair(p.rowadd + (long)bidx[hh] * p.ldra + n0 + c);
-              x0 += f.x;
-              x1 += f.y;
-            }
-            if (do_silu) {
-              x0 = silu_f(x0);
-              x1 = silu_f(x1);
-            } else if (do_gelu) {
-              x0 = gelu_erf_f(x0);
-              x1 = gelu_erf_f(x1);
-            }
+          x0 *= gelu_erf_f(g0);
+          x1 *= gelu_erf_f(g1);
+        } else {
+          if (!gated && p.rowadd && rok[hh] && out_col_base + 8 * j < n_out_total) {
+            const float2 f = ld_pair(p.rowadd + (long)bidx[hh] * p.ldra + n0 + 8 * j + 2 * t4);
+            x0 += f.x;
+            x1 += f.y;
           }
-          if (nchw) {
-            float* o = reinterpret_cast<float*>(p.out);
-            const long hw = p.conv ? (long)p.H * p.W : (long)p.rows_per_batch;
+          if (do_silu) {
+            x0 = silu_f(x0);
+            x1 = silu_f(x1);
+          } else if (do_gelu) {
+            x0 = gelu_erf_f(x0);
+            x1 = gelu_erf_f(x1);
+          }
+        }
+      };
+      if constexpr (nchw) {
+        // fp32 NCHW (the final conv, one launch per forward): stored straight from the fragments
+        float* o = reinterpret_cast<float*>(p.out);
+        const long hw = p.conv ? (long)p.H * p.W : (long)p.rows_per_batch;
+#pragma unroll
+        for (int j = 0; j < NJO; ++j) {
+          const int oc = out_col_base + 8 * j + 2 * t4;
+          if (oc >= n_out_total) continue;
+          float2 bv, bg, sv, sgt;
+          col_vecs(j, bv, bg, sv, sgt);
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            if (!rok[hh]) continue;
+            float x0, x1;
+            act_pair(j, hh, bv, bg, sv, sgt, x0, x1);
             o[((long)bidx[hh] * n_out_total + oc) * hw + pix[hh]] = x0;
-            if (hi) o[((long)bidx[hh] * n_out_total + oc + 1) * hw + pix[hh]] = x1;
-          } else {
-            if (has_res) {
-              const float2 r = ld_pair(p.residual + orow[hh] * p.ldr + oc);
-              const float g = gated ? gate_r[hh] : gate;
-              x0 = fmaf(g, x0, r.x);
-              x1 = fmaf(g, x1, r.y);
-            }
-            if (lno) {
-              ln_ps[hh] += x0 + x1;
-              ln_pq[hh] = fmaf(x0, x0, fmaf(x1, x1, ln_pq[hh]));
-            }
-            *reinterpret_cast<uint32_t*>(reinterpret_cast<h16*>(p.out) + orow[hh] * p.ldo + oc) = pack_half2(x0, x1);
+            if (oc + 1 < n_out_total) o[((long)bidx[hh] * n_out_total + oc + 1) * hw + pix[hh]] = x1;
           }
+        }
+      } else {
+        // 16-bit output, staged in sE: one ldmatrix / stmatrix x4 covers the groups j = 2 jp, 2 jp + 1 of both row
+        // halves (matrix 2u + hh = group 2 jp + u, rows 8 hh ..); lane l gives the address of row l % 8 of matrix l / 8.
+        // Rows past M / past the conv image and columns past N are computed on whatever sE holds and clipped by
+        // the TMA store.
+        const int lrow = cw * 64 + (warp & 3) * 16 + 8 * ((lane >> 3) & 1) + (lane & 7);
+        const uint32_t se = smem_u32(sE);
+        mbar_wait(epi_ready, ep);
+        ep ^= 1;
+#pragma unroll
+        for (int jp = 0; jp < NJO / 2; ++jp) {
+          const uint32_t addr = se + epi_offset(lrow, 2 * jp + (lane >> 4));
+          uint32_t rr[4] = {0u, 0u, 0u, 0u};
+          if (has_res) ldmatrix_x4(rr, addr);
+          uint32_t packed[4];
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            const int j = 2 * jp + u;
+            const bool cok = out_col_base + 8 * j < n_out_total;
+            float2 bv, bg, sv, sgt;
+            col_vecs(j, bv, bg, sv, sgt);
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              float x0, x1;
+              act_pair(j, hh, bv, bg, sv, sgt, x0, x1);
+              if (has_res) {
+                const float2 r = unpack_half2(rr[2 * u + hh]);
+                const float g = gated ? gate_r[hh] : gate;
+                x0 = fmaf(g, x0, r.x);
+                x1 = fmaf(g, x1, r.y);
+              }
+              if (lno && cok) {
+                ln_ps[hh] += x0 + x1;
+                ln_pq[hh] = fmaf(x0, x0, fmaf(x1, x1, ln_pq[hh]));
+              }
+              packed[2 * u + hh] = pack_half2(x0, x1);
+            }
+          }
+          stmatrix_x4(addr, packed);
+        }
+        fence_proxy_async_smem();  // the stmatrix writes -> visible to the TMA store
+        named_bar_sync(1, 256);
+        if (ct == 0) {
+          mbar_arrive(epi_full);
+          stamp_tile(2);
         }
       }
       // LayerNorm fold, producer side: the row's (sum, sumsq) over this tile's columns, slot = n tile
@@ -492,9 +618,25 @@ static void choose_patch(int H, int W, int* PW, int* PH, int* PB) {
   *PB = 128 / (pw * ph);
 }
 
+// Tensor map of a 16-bit epilogue operand (the output, or the residual) with `n` columns and row stride `ld`
+// elements, in boxes of one epilogue slab: (32 columns, 128 rows) for a linear layer, (32, PW, PH, PB) over
+// the NHWC image for conv3x3 -- the rows of the tile's A patch.  Its bounds clip the boxes of edge tiles.
+static int encode_epi_map(CUtensorMap* m, const void* base, int n, int ld, const idiff_gemm_args* a, const Params& p) {
+  if (p.conv) {
+    const uint64_t dims[4] = {(uint64_t)n, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.Bn};
+    const uint64_t strides[3] = {(uint64_t)ld * 2, (uint64_t)p.W * ld * 2, (uint64_t)p.H * p.W * ld * 2};
+    const uint32_t box[4] = {(uint32_t)EPI_SLAB_COLS, (uint32_t)p.PW, (uint32_t)p.PH, (uint32_t)p.PB};
+    return encode_tmap_f16_sw(m, base, 4, dims, strides, box, 64);
+  }
+  const uint64_t dims[2] = {(uint64_t)n, (uint64_t)a->M};
+  const uint64_t strides[1] = {(uint64_t)ld * 2};
+  const uint32_t box[2] = {(uint32_t)EPI_SLAB_COLS, (uint32_t)BM};
+  return encode_tmap_f16_sw(m, base, 2, dims, strides, box, 64);
+}
+
 template <int BN, int MODE>
 static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
-  using C = Cfg<BN>;
+  using C = Cfg<BN, MODE>;
   Params p;
   memset(&p, 0, sizeof(p));
   p.M = a->M;
@@ -556,6 +698,13 @@ static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
   }
   p.n_tiles = (a->N + BN - 1) / BN;
   p.T = p.n_tiles * m_tiles;
+  CUtensorMap tmO, tmR;
+  memset(&tmO, 0, sizeof(tmO));
+  memset(&tmR, 0, sizeof(tmR));
+  if (C::EW > 0) {
+    if (encode_epi_map(&tmO, a->out, MODE == MODE_GEGLU ? a->N / 2 : a->N, a->ldo, a, p)) return -1;
+    if (a->residual && encode_epi_map(&tmR, a->residual, a->N, a->ldr, a, p)) return -1;
+  }
 
   if (g_num_sms == 0) {
     int dev = 0;
@@ -591,7 +740,7 @@ static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
                                           C::SMEM_BYTES));
     attr_set = true;
   }
-  IDIFF_CHECK_CUDA(launch_pdl(gemm2_kernel<BN, MODE>, dim3(p.G), dim3(THREADS), C::SMEM_BYTES, stream, tmA, tmB, p));
+  IDIFF_CHECK_CUDA(launch_pdl(gemm2_kernel<BN, MODE>, dim3(p.G), dim3(THREADS), C::SMEM_BYTES, stream, tmA, tmB, tmO, tmR, p));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -784,7 +933,9 @@ extern "C" int idiff_set_gemm_workspace(void* ptr, long bytes) {
 }
 
 // Debug / profiling hook: when set, every GEMM CTA writes %globaltimer stamps to trace[cta*16 ..]: slot 0
-// kernel entry, slot 7 exit, slots 12 / 13 the SM clock at entry / exit; the other slots stay 0.  NULL disables.
+// kernel entry, slot 7 exit, slots 12 / 13 the SM clock at entry / exit; for the CTA's first epilogue tile
+// slots 1 / 2 / 3 = mainloop done / epilogue staged in shared memory / TMA store issued, slots 4 / 5 / 6 the
+// same for its last one (a CTA without an epilogue tile leaves them 0).  NULL disables.
 extern "C" int idiff_set_gemm_trace(void* ptr) {
   idiff::v2::g_trace = reinterpret_cast<unsigned long long*>(ptr);
   return 0;

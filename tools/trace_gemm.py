@@ -21,9 +21,9 @@ shapes = {
     "ff2_1280_8": lambda: (r(B * 64, 5120), r(1280, 5120, sc=0.02), dict(residual=r(B * 64, 1280))),
     "conv320": lambda: (r(B * 4096, 320), r(320, 2880, sc=0.02), dict(conv=(B, 64, 64, 320), residual=r(B * 4096, 320))),
 }
-names = ["entry", "1st tile", "seg0 issued", "acc0 ready", "fixup done", "epi0 done", "loops done", "exit",
-         "c0 start", "c0 computed", "c0 staged", "c0 store issued", "c1 start", "c1 computed", "c1 staged",
-         "c1 store issued"]
+# slots written by gemm2_kernel (gemm2.cu, idiff_set_gemm_trace): 1-3 the CTA's first epilogue tile, 4-6 its last
+names = ["entry", "tile0 mainloop", "tile0 staged", "tile0 stored", "last mainloop", "last staged", "last stored",
+         "exit"]
 lib = _lib.load()
 trace = torch.zeros(256 * 16, dtype=torch.int64, device=dev)
 for name in sys.argv[1:]:
@@ -45,9 +45,7 @@ for name in sys.argv[1:]:
     rel = (t - t0).float() / 1e3  # us
     mhz = ((t[:, 13] - t[:, 12]).float() / (t[:, 7] - t[:, 0]).float().clamp(min=1) * 1e3).median()
     print(f"== {name}: {t.shape[0]} CTAs, kernel span {rel[:, 7].max():.1f} us, SM clock during kernel ~{mhz:.0f} MHz")
-    names[14] = "c0 tmem loaded"
-    names[15] = "c1 start"
-    for i, n in list(enumerate(names[:12])) + [(14, names[14]), (15, names[15])]:
+    for i, n in enumerate(names):
         col = rel[:, i][t[:, i] > 0]
         if col.numel():
             print(f"   {n:16s} min {col.min():7.2f}  median {col.median():7.2f}  max {col.max():7.2f} us")
