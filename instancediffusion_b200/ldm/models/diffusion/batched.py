@@ -8,6 +8,8 @@ schedule) and first-conv state.  Per request the arithmetic is that of its own s
 PLMS updates are `PLMSBase._step_predict` / `_step_finish` on its own trajectories with its own guidance scale,
 and a Multi-instance request merges its latents with `ops.latent_mean` at its own step int(steps * mis), where
 steps is the length of the PLMS schedule (`schedule_steps`: S + 1 for some S, e.g. 31 for S = 30), as there.
+That per-request machinery is `_RequestState`, which `SamplingEngine` (engine.py) drives too: `sample_requests` is
+the lock-step driver on top of it.
 
 Contract: each returned latent equals, within floating-point tolerance, what `PLMSSampler.sample()` (input dict,
 mis = 0) or `PLMSSamplerInst.sample()` (input list [global, instance_1 .. instance_n]) returns for that request
@@ -16,6 +18,7 @@ first-conv swap are what a sequential run of the same requests would leave.
 """
 from __future__ import annotations
 
+from contextlib import contextmanager
 from dataclasses import dataclass
 from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
 
@@ -145,67 +148,175 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
     return plans
 
 
-class _State:
-    """Per-request sampling state."""
+class _RequestState:
+    """One request being sampled by `sample_requests` or `SamplingEngine`: its plan and its own PLMS schedule
+    (`make_schedule(S)`), what the model was when the request was admitted, and, once started, its trajectories and its
+    position in the schedule.  Both drivers evaluate a request the same way: `begin`, one forward of its trajectories at
+    `fuser_scale()` and `conv_flag(...)`, `advance` with the eps; after the last step `finish` returns its latent."""
 
-    def __init__(self, req: Request, plan: RequestPlan, S: int, device):
+    def __init__(self, req: Request, plan: RequestPlan, S: int, model, diffusion):
         self.req, self.plan = req, plan
+        self.base = PLMSBase(diffusion, model)
+        self.base.make_schedule(ddim_num_steps=int(S))
+        self.time_range = np.flip(self.base.ddim_timesteps)
+        self.steps = len(self.time_range)
+        self.alphas = req.alpha_generator_func(self.steps) if req.alpha_generator_func is not None else None
+        self.scale = 0.0  # without an alpha schedule: the model's fuser scale at admission
+        if self.alphas is None:
+            fusers = [m for m in model.modules() if isinstance(m, GatedSelfAttentionDense)]
+            self.scale = float(fusers[0].scale) if fusers else 0.0
+            if any(float(f.scale) != self.scale for f in fusers):
+                raise ValueError("requests without an alpha_generator_func run at the model's fuser scale, "
+                                 "which differs between fusers")
+        self.restored = bool(getattr(model, "_first_conv_restored", False))
+        # uncond inputs: the null grounding tokens of the request's batch (UNetModel.object_kv(None) uses the batch
+        # the grounding tokenizer input was last prepared with, which serves batch 1 and that batch)
+        gti = getattr(model, "grounding_tokenizer_input", None)
+        own = gti is None or not getattr(gti, "set", False) or gti.batch in (1, plan.images)
+        self.null_input = None if own else gti.get_null_input(batch=plan.images)
         ins = _inputs_of(req)
+        x = next((i["x"] for i in ins if i.get("x") is not None), None)
+        self.group = (tuple(x.shape[2:]) if x is not None else tuple(req.shape[2:]), ins[0]["context"].shape[1])
+        self.trajs: List[Trajectory] = []
+        self.gs = float(req.guidance_scale)
+        self.reached_zero = False
+        self.i = 0             # current step
+        self.pending = None    # predictor state while the corrector's evaluation is due
+        self.ts_next = None
+
+    def start(self):
+        """The trajectories, when the request starts sampling."""
+        ins = _inputs_of(self.req)
         if ins[0].get("x") is None:  # as the samplers: one noise tensor shared by every trajectory
-            img = torch.randn(tuple(req.shape), device=device)
+            img = torch.randn(tuple(self.req.shape), device=self.base.device)
             for inp in ins:
                 inp["x"] = img
         self.trajs = [Trajectory(inp) for inp in ins]
-        self.alphas = req.alpha_generator_func(S) if req.alpha_generator_func is not None else None
-        self.reached_zero = False
-        self.gs = float(req.guidance_scale)
+
+    def images(self) -> int:
+        """Images the request puts into an evaluation before its merge."""
+        return self.plan.trajectories * self.plan.rows()
+
+    def inputs(self) -> List[dict]:
+        """Every input dict the request's forwards use: its trajectories and its uncond branch."""
+        ins = list(_inputs_of(self.req))
+        if self.plan.cfg:
+            ins.append(dict(context=self.req.uc, grounding_input=self.null_input))
+        return ins
 
     def merge(self):
         """Multi-instance merge: the global trajectory continues from the mean of the n+1 latents
-        (plms_instance.py:135)."""
-        xs = [tr.input["x"].float().contiguous() for tr in self.trajs]
-        merged = torch.empty_like(xs[0])
-        ops.latent_mean(xs, merged)
-        self.trajs[0].input["x"] = merged
-        self.trajs = self.trajs[:1]
+        (plms_instance.py:135).  A single trajectory is left as it is."""
+        if len(self.trajs) > 1:
+            xs = [tr.input["x"].float().contiguous() for tr in self.trajs]
+            merged = torch.empty_like(xs[0])
+            ops.latent_mean(xs, merged)
+            self.trajs[0].input["x"] = merged
+            self.trajs = self.trajs[:1]
 
+    def begin(self):
+        """Before an evaluation: the merge due before step i and the timesteps of step i, unless the evaluation is the
+        corrector's of the first PLMS step (the predictor left the inputs at t_next)."""
+        if self.pending is None:
+            if self.plan.merge_step == self.i:
+                self.merge()
+            ts, self.ts_next = self.base._timesteps(self.plan.images, self.i, self.time_range)
+            for tr in self.trajs:
+                tr.input["timesteps"] = ts
 
-def _evaluate(model, states: List[_State], chunks: Sequence[Tuple[List[Tuple[int, int]], Optional[int]]], scales,
-              restored, null_inputs, per_image_conv: bool = False):
-    """One UNet evaluation of the trajectories of `chunks`, one forward per (chunk, padded size): {(request, trajectory):
-    (e_c, e_u|None)}.  A chunk with a padded size is filled up to it with copies of its last input (same context and
-    grounding, so its hoisted tensors come from the caches) with a zero latent, fuser scale 0 and the model's own
-    conv; their outputs are dropped.  per_image_conv: see UNetModel.forward_batched."""
-    out = {}
-    for chunk, padded in chunks:
-        inputs, sc, rs = [], [], []
-        for r, k in chunk:
-            st = states[r]
-            tr = st.trajs[k]
-            inputs.append(tr.input)
-            if st.plan.cfg:
-                inputs.append(dict(x=tr.input["x"], timesteps=tr.input["timesteps"], context=st.req.uc,
-                                   grounding_input=null_inputs[r]))
-            n = 2 if st.plan.cfg else 1
-            sc += [scales[r]] * n
-            rs += [restored[r]] * n
-        if padded is not None:
-            last = inputs[-1]
-            pad = dict(last, x=torch.zeros_like(last["x"]))
-            n_pad = (padded - sum(i["x"].shape[0] for i in inputs)) // last["x"].shape[0]
-            inputs += [pad] * n_pad
-            sc += [0.0] * n_pad
-            rs += [False] * n_pad
-        outs = model.forward_batched(inputs, scales=sc, restored=rs, per_image_conv=per_image_conv)
-        j = 0
-        for r, k in chunk:
-            if states[r].plan.cfg:
-                out[(r, k)] = (outs[j], outs[j + 1])
-                j += 2
-            else:
-                out[(r, k)] = (outs[j], None)
-                j += 1
-    return out
+    def fuser_scale(self) -> float:
+        """Fuser scale of step i.  Sets `reached_zero` from the first alpha 0 on: there the request's own sampler
+        swaps in the SD1.5 conv (PLMSBase._set_alpha)."""
+        if self.alphas is None:
+            return self.scale
+        alpha = float(self.alphas[self.i])
+        self.reached_zero |= alpha == 0
+        return alpha
+
+    def conv_flag(self, sd_conv: bool) -> bool:
+        """Whether the request's images take the SD1.5 conv: the model had it at admission, or the request reached
+        alpha 0 and `sd_conv` says the model has that conv to give."""
+        return self.restored or (self.reached_zero and sd_conv)
+
+    def advance(self, evals):
+        """Advance by an evaluation's [(e_c, e_u|None)] per trajectory: the predictor of a first PLMS step, which
+        leaves `pending` set until the corrector's evaluation, or the corrector or a plain step, which moves to step
+        i + 1."""
+        index = self.steps - self.i - 1
+        pending, self.pending = self.pending, None
+        if pending is None:
+            self.pending = self.base._step_predict(self.trajs, evals, self.ts_next, index, self.gs)
+            if self.pending is not None:
+                return
+        self.base._step_finish(self.trajs, evals, pending, index, self.gs)
+        self.i += 1
+
+    def finish(self) -> torch.Tensor:
+        """The latent, after the last step and, for mis = 1, the merge that follows it."""
+        if self.plan.merge_step == self.steps:
+            self.merge()
+        return self.trajs[0].input["x"]
+
+    @staticmethod
+    def evaluate(model, states: Sequence[_RequestState], forwards: Sequence[Tuple[List[Tuple[int, int]], Optional[int]]],
+                 scales: Sequence[float], flags: Sequence[bool], per_image_conv: bool = False):
+        """One UNet evaluation of the trajectories of `forwards`, one forward per (chunk of (request, trajectory) slots,
+        padded size), each request's images at its fuser scale and conv flag: {(request, trajectory): (e_c, e_u|None)}.
+        A chunk with a padded size is filled up to it with copies of its last input (same context and grounding, so
+        its hoisted tensors come from the caches) with a zero latent, fuser scale 0 and the model's own conv; their
+        outputs are dropped.  per_image_conv: see UNetModel.forward_batched."""
+        out = {}
+        for chunk, padded in forwards:
+            inputs, sc, rs = [], [], []
+            for r, k in chunk:
+                st = states[r]
+                tr = st.trajs[k]
+                inputs.append(tr.input)
+                if st.plan.cfg:
+                    inputs.append(dict(x=tr.input["x"], timesteps=tr.input["timesteps"], context=st.req.uc,
+                                       grounding_input=st.null_input))
+                n = 2 if st.plan.cfg else 1
+                sc += [scales[r]] * n
+                rs += [flags[r]] * n
+            if padded is not None:
+                last = inputs[-1]
+                pad = dict(last, x=torch.zeros_like(last["x"]))
+                n_pad = (padded - sum(i["x"].shape[0] for i in inputs)) // last["x"].shape[0]
+                inputs += [pad] * n_pad
+                sc += [0.0] * n_pad
+                rs += [False] * n_pad
+            outs = model.forward_batched(inputs, scales=sc, restored=rs, per_image_conv=per_image_conv)
+            j = 0
+            for r, k in chunk:
+                if states[r].plan.cfg:
+                    out[(r, k)] = (outs[j], outs[j + 1])
+                    j += 2
+                else:
+                    out[(r, k)] = (outs[j], None)
+                    j += 1
+        return out
+
+    @staticmethod
+    @contextmanager
+    def cache_bounds(model, hoist: int, cat: int, graph_pool=None):
+        """Within the block, the model's hoisted-tensor caches hold at least `hoist` text / object K/V entries and `cat`
+        concatenations and, if given, new CUDA-graph captures use `graph_pool`; afterwards the model has its own
+        values again."""
+        bounds = {"hoist_cache_entries": max(hoist, getattr(model, "hoist_cache_entries", 0)),
+                  "cat_cache_entries": max(cat, getattr(model, "cat_cache_entries", 0))}
+        if graph_pool is not None:
+            bounds["graph_pool"] = graph_pool
+        saved = {k: model.__dict__[k] for k in bounds if k in model.__dict__}
+        for k, v in bounds.items():
+            setattr(model, k, v)
+        try:
+            yield
+        finally:
+            for k in bounds:
+                if k in saved:
+                    setattr(model, k, saved[k])
+                else:
+                    delattr(model, k)
 
 
 @torch.no_grad()
@@ -222,88 +333,39 @@ def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], 
     from ....utils.model import set_alpha_scale
     reqs = [r if isinstance(r, Request) else Request(**r) for r in requests]
     plans = check_requests(reqs, S, max_batch, diffusion.num_timesteps)
-    base = PLMSBase(diffusion, model)
-    base.make_schedule(ddim_num_steps=S)
-    time_range = np.flip(base.ddim_timesteps)
-    total = base.ddim_timesteps.shape[0]
-    assert total == schedule_steps(S, diffusion.num_timesteps)
-    states = [_State(r, p, len(time_range), base.device) for r, p in zip(reqs, plans)]
-
-    fusers = [m for m in model.modules() if isinstance(m, GatedSelfAttentionDense)]
-    entry_scale = float(fusers[0].scale) if fusers else 0.0
-    if any(s.alphas is None for s in states) and any(float(f.scale) != entry_scale for f in fusers):
-        raise ValueError("requests without an alpha_generator_func run at the model's fuser scale, "
-                         "which differs between fusers")
-    entry_restored = bool(getattr(model, "_first_conv_restored", False))
-    # uncond inputs: the null grounding tokens of the request's batch (UNetModel.object_kv(None) uses the batch
-    # the grounding tokenizer input was last prepared with, which serves batch 1 and that batch)
-    gti = getattr(model, "grounding_tokenizer_input", None)
-    null_inputs = []
-    for p in plans:
-        own = gti is None or not getattr(gti, "set", False) or gti.batch in (1, p.images)
-        null_inputs.append(None if own else gti.get_null_input(batch=p.images))
-
-    # the model's hoisted-tensor caches must hold every input and every chunk combination of the run, or each
-    # forward recomputes its text / object K/V: raised for the run, restored afterwards
-    chunks = {tuple(c) for i in range(len(time_range)) for c in plan_step(plans, i, max_batch)}
-    bounds = {"hoist_cache_entries": sum(p.trajectories + 2 for p in plans) + 8, "cat_cache_entries": 2 * len(chunks) + 2}
-    saved = {k: model.__dict__[k] for k in bounds if k in model.__dict__}
-    for k, v in bounds.items():
-        setattr(model, k, max(v, getattr(model, k, 0)))
-    try:
-        _run(model, base, states, time_range, total, max_batch, entry_scale, entry_restored, null_inputs)
-    finally:
-        for k in bounds:
-            if k in saved:
-                setattr(model, k, saved[k])
-            else:
-                delattr(model, k)
-        model.trim_hoisted()  # the run's concatenations (hundreds of MB each) do not outlive it
-
+    states = [_RequestState(r, p, S, model, diffusion) for r, p in zip(reqs, plans)]
     for st in states:
-        if st.plan.merge_step == len(time_range):  # mis = 1: the merge follows the last step
-            st.merge()
+        st.start()
+    steps = states[0].steps
+    # the model's hoisted-tensor caches must hold every input and every chunk combination of the run, or each
+    # forward recomputes its text / object K/V: raised for the run
+    chunks = {tuple(c) for i in range(steps) for c in plan_step(plans, i, max_batch)}
+    try:
+        with _RequestState.cache_bounds(model, sum(p.trajectories + 2 for p in plans) + 8, 2 * len(chunks) + 2):
+            for _ in range(steps):
+                scales = []
+                for st in states:
+                    st.begin()
+                    zero = st.reached_zero
+                    scales.append(st.fuser_scale())
+                    if st.reached_zero and not zero:
+                        model.restore_first_conv_from_SD()  # the swap a run of this request makes here
+                sd_conv = bool(getattr(model, "_first_conv_restored", False))
+                flags = [st.conv_flag(sd_conv) for st in states]
+                todo = range(len(states))
+                while todo:  # every request's step, then the corrector's evaluation of a first PLMS step
+                    slots = [(r, k) for r in todo for k in range(len(states[r].trajs))]
+                    forwards = [(c, None) for c in plan_chunks(slots, plans, max_batch)]
+                    evals = _RequestState.evaluate(model, states, forwards, scales, flags)
+                    for r in todo:
+                        states[r].advance([evals[(r, k)] for k in range(len(states[r].trajs))])
+                    todo = [r for r in todo if states[r].pending is not None]
+    finally:
+        model.trim_hoisted()  # the run's concatenations (hundreds of MB each) do not outlive it
+    latents = [st.finish() for st in states]
     # the model's fuser scale as a sequential run leaves it: the last alpha of the last request that sets one
     for st in reversed(states):
         if st.alphas is not None:
             set_alpha_scale(model, st.alphas[-1])
             break
-    return [st.trajs[0].input["x"] for st in states]
-
-
-def _run(model, base, states, time_range, total, max_batch, entry_scale, entry_restored, null_inputs):
-    """The S steps of sample_requests."""
-    for i in range(len(time_range)):
-        index = total - i - 1
-        scales, restored = [], []
-        for st in states:
-            if st.plan.merge_step == i:
-                st.merge()
-            alpha = st.alphas[i] if st.alphas is not None else entry_scale
-            if st.alphas is not None and alpha == 0 and not st.reached_zero:
-                st.reached_zero = True
-                model.restore_first_conv_from_SD()  # the swap a run of this request makes here (PLMSBase._set_alpha)
-            scales.append(float(alpha))
-        model_restored = bool(getattr(model, "_first_conv_restored", False))
-        for st in states:
-            restored.append(entry_restored or (st.reached_zero and model_restored))
-        steps = {}
-        for r, st in enumerate(states):
-            ts, ts_next = base._timesteps(st.plan.images, i, time_range)
-            steps[r] = ts_next
-            for tr in st.trajs:
-                tr.input["timesteps"] = ts
-        slots = [(r, k) for r, st in enumerate(states) for k in range(len(st.trajs))]
-        plans = [st.plan for st in states]
-        evals = _evaluate(model, states, [(c, None) for c in plan_chunks(slots, plans, max_batch)], scales, restored,
-                          null_inputs)
-        pending = {}
-        for r, st in enumerate(states):
-            pending[r] = base._step_predict(st.trajs, [evals[(r, k)] for k in range(len(st.trajs))], steps[r], index,
-                                            st.gs)
-        again = [(r, k) for r, k in slots if pending[r] is not None]
-        if again:  # first step of a trajectory: the corrector's evaluation at t_next
-            evals.update(_evaluate(model, states, [(c, None) for c in plan_chunks(again, plans, max_batch)], scales,
-                                   restored, null_inputs))
-        for r, st in enumerate(states):
-            base._step_finish(st.trajs, [evals[(r, k)] for k in range(len(st.trajs))], pending[r], index, st.gs)
+    return latents

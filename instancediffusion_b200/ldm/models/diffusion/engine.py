@@ -10,9 +10,10 @@ when the slowest one finishes.  `SamplingEngine` lets requests join and leave be
 
 A tick gives every live trajectory exactly one UNet evaluation: the one at t of its current step or, for a request
 in the Euler predictor of its first PLMS step, the corrector's evaluation at t_next (so the corrector rides in the
-next tick with everyone else).  Per request the arithmetic is that of its own sampler, on its own schedule
-(`PLMSBase.make_schedule(S)`): history and updates are `PLMSBase._step_predict` / `_step_finish`, and a
-Multi-instance request merges before its step int(schedule_steps(S) * mis), after the last one for mis = 1.
+next tick with everyone else).  Each request is a `batched._RequestState`, the per-request sampling state that
+`sample_requests` drives too: its own schedule (`PLMSBase.make_schedule(S)`), its sampler's arithmetic
+(`PLMSBase._step_predict` / `_step_finish`) and its Multi-instance merge before step int(schedule_steps(S) * mis),
+after the last one for mis = 1.  The engine adds admission, the grouping of a tick's forwards and retirement.
 
 The evaluations of a tick are grouped by (latent H x W, context length) in admission order, split into forwards of
 at most `max_batch` images by `plan_chunks`, and each forward is padded to the smallest of `buckets` that holds it.
@@ -30,12 +31,9 @@ from __future__ import annotations
 from collections import deque
 from typing import Dict, List, Optional, Sequence, Tuple, Union
 
-import numpy as np
 import torch
 
-from ...modules.attention import GatedSelfAttentionDense
-from ._plms_common import PLMSBase
-from .batched import Request, RequestPlan, _State, _evaluate, _inputs_of, check_requests, plan_chunks
+from .batched import Request, RequestPlan, _RequestState, check_requests, plan_chunks
 
 
 def pick_bucket(images: int, unit: int, buckets: Optional[Sequence[int]]) -> Optional[int]:
@@ -63,33 +61,6 @@ def plan_forwards(slots: Sequence[Tuple[int, int]], plans: Sequence[RequestPlan]
     return out
 
 
-class _Live:
-    """A submitted request: its plan, its own schedule and, once admitted, its sampling state and position."""
-
-    def __init__(self, ticket: int, req: Request, plan: RequestPlan, base: PLMSBase, scale: float, restored: bool,
-                 null_input, group: tuple):
-        self.ticket, self.req, self.plan, self.base = ticket, req, plan, base
-        self.time_range = np.flip(base.ddim_timesteps)
-        self.steps = len(self.time_range)
-        self.scale, self.restored = scale, restored  # fuser scale / first-conv state of the model at submit
-        self.null_input, self.group = null_input, group
-        self.state: Optional[_State] = None
-        self.i = 0               # current step
-        self.pending = None      # predictor state while the corrector evaluation is due
-        self.ts_next = None
-
-    def images(self) -> int:
-        """Images this request puts into a tick's forwards (its trajectories before the merge)."""
-        return self.plan.trajectories * self.plan.rows()
-
-    def inputs(self) -> List[dict]:
-        """Every input dict the request's forwards use: its trajectories and its uncond branch."""
-        ins = list(_inputs_of(self.req))
-        if self.plan.cfg:
-            ins.append(dict(context=self.req.uc, grounding_input=self.null_input))
-        return ins
-
-
 class SamplingEngine:
     """Step-level scheduler of sampling requests on one model.  `max_batch`: images per UNet forward;
     `max_live_images`: bound of the images of the admitted requests (default 4 * max_batch); `buckets`: the padded
@@ -112,8 +83,8 @@ class SamplingEngine:
         self.buckets = buckets
         self.share_graph_pool = bool(share_graph_pool)
         self._pool = None
-        self._queue: deque = deque()
-        self._live: List[_Live] = []
+        self._queue: deque = deque()                     # (ticket, state), in submission order
+        self._live: Dict[int, _RequestState] = {}        # ticket -> state, in admission order
         self._next = 0
         self.graphs_captured = 0
         self.forwards = 0        # UNet forwards run
@@ -121,11 +92,11 @@ class SamplingEngine:
 
     @property
     def queued(self) -> List[int]:
-        return [e.ticket for e in self._queue]
+        return [t for t, _ in self._queue]
 
     @property
     def live(self) -> List[int]:
-        return [e.ticket for e in self._live]
+        return list(self._live)
 
     # --------------------------------------------------------------------------------------------
     def submit(self, request: Union[Request, dict]) -> int:
@@ -139,28 +110,10 @@ class SamplingEngine:
         if size > self.max_live_images:
             raise ValueError(f"request of {size} images (trajectories x images x CFG) exceeds max_live_images="
                              f"{self.max_live_images}")
-        model = self.model
-        scale = 0.0
-        if req.alpha_generator_func is None:  # runs at the model's fuser scale, as set when submitted
-            fusers = [m for m in model.modules() if isinstance(m, GatedSelfAttentionDense)]
-            scale = float(fusers[0].scale) if fusers else 0.0
-            if any(float(f.scale) != scale for f in fusers):
-                raise ValueError("requests without an alpha_generator_func run at the model's fuser scale, "
-                                 "which differs between fusers")
-        restored = bool(getattr(model, "_first_conv_restored", False))
-        # uncond inputs: the null grounding tokens of the request's batch (as sample_requests)
-        gti = getattr(model, "grounding_tokenizer_input", None)
-        own = gti is None or not getattr(gti, "set", False) or gti.batch in (1, plan.images)
-        null_input = None if own else gti.get_null_input(batch=plan.images)
-        ins = _inputs_of(req)
-        x = next((i["x"] for i in ins if i.get("x") is not None), None)
-        hw = tuple(x.shape[2:]) if x is not None else tuple(req.shape[2:])
-        base = PLMSBase(self.diffusion, model)
-        base.make_schedule(ddim_num_steps=int(req.S))
-        e = _Live(self._next, req, plan, base, scale, restored, null_input, (hw, ins[0]["context"].shape[1]))
-        self._next += 1
-        self._queue.append(e)
-        return e.ticket
+        st = _RequestState(req, plan, int(req.S), self.model, self.diffusion)
+        ticket, self._next = self._next, self._next + 1
+        self._queue.append((ticket, st))
+        return ticket
 
     def drain(self) -> Dict[int, torch.Tensor]:
         """Tick until nothing is queued or live; the latents of every request that finished meanwhile."""
@@ -172,87 +125,47 @@ class SamplingEngine:
     @torch.no_grad()
     def step(self) -> Dict[int, torch.Tensor]:
         """One tick: admit, evaluate every live trajectory once, advance; {ticket: latent} of the finished requests."""
-        live_images = sum(e.images() for e in self._live)
-        while self._queue and live_images + self._queue[0].images() <= self.max_live_images:
-            e = self._queue.popleft()
-            e.state = _State(e.req, e.plan, e.steps, e.base.device)
-            self._live.append(e)
-            live_images += e.images()
+        live_images = sum(st.images() for st in self._live.values())
+        while self._queue and live_images + self._queue[0][1].images() <= self.max_live_images:
+            ticket, st = self._queue.popleft()
+            st.start()
+            self._live[ticket] = st
+            live_images += st.images()
         if not self._live:
             return {}
-        restorable = getattr(self.model, "first_conv_restorable", True)
-        scales, restored = [], []
-        for e in self._live:
-            st = e.state
-            if e.pending is None:
-                if e.plan.merge_step == e.i and len(st.trajs) > 1:
-                    st.merge()
-                ts, e.ts_next = e.base._timesteps(e.plan.images, e.i, e.time_range)
-                for tr in st.trajs:
-                    tr.input["timesteps"] = ts
-            alpha = st.alphas[e.i] if st.alphas is not None else e.scale
-            if st.alphas is not None and alpha == 0:
-                st.reached_zero = True  # the step where its own sampler swaps in the SD1.5 conv
-            scales.append(float(alpha))
-            restored.append(e.restored or (st.reached_zero and restorable))
-        states = [e.state for e in self._live]
+        states = list(self._live.values())
+        sd_conv = getattr(self.model, "first_conv_restorable", True)
+        scales, flags = [], []
+        for st in states:
+            st.begin()
+            scales.append(st.fuser_scale())
+            flags.append(st.conv_flag(sd_conv))
         slots = [(r, k) for r, st in enumerate(states) for k in range(len(st.trajs))]
-        forwards = plan_forwards(slots, [st.plan for st in states], [e.group for e in self._live], self.max_batch,
+        forwards = plan_forwards(slots, [st.plan for st in states], [st.group for st in states], self.max_batch,
                                  self.buckets)
-        evals = self._run(states, forwards, scales, restored)
+        evals = self._run(states, forwards, scales, flags)
 
-        done, still = {}, []
-        for r, e in enumerate(self._live):
-            st = e.state
-            ev = [evals[(r, k)] for k in range(len(st.trajs))]
-            index = e.steps - e.i - 1
-            if e.pending is not None:  # the corrector of the first PLMS step
-                e.base._step_finish(st.trajs, ev, e.pending, index, st.gs)
-                e.pending = None
-            else:
-                e.pending = e.base._step_predict(st.trajs, ev, e.ts_next, index, st.gs)
-                if e.pending is not None:  # the corrector's evaluation at t_next comes next tick
-                    still.append(e)
-                    continue
-                e.base._step_finish(st.trajs, ev, None, index, st.gs)
-            e.i += 1
-            if e.i < e.steps:
-                still.append(e)
-                continue
-            if e.plan.merge_step == e.steps and len(st.trajs) > 1:  # mis = 1: the merge follows the last step
-                st.merge()
-            done[e.ticket] = st.trajs[0].input["x"]
-        finished = [e for e in self._live if e.ticket in done]
-        self._live = still
+        done = {}
+        for r, (ticket, st) in enumerate(list(self._live.items())):
+            st.advance([evals[(r, k)] for k in range(len(st.trajs))])
+            if st.i == st.steps:
+                done[ticket] = st.finish()
+        finished = [self._live.pop(t) for t in done]
         if finished:
-            keep = [i for e in list(self._live) + list(self._queue) for i in e.inputs()]
-            self.model.drop_hoisted([i for e in finished for i in e.inputs()], keep)
+            keep = [i for st in list(self._live.values()) + [st for _, st in self._queue] for i in st.inputs()]
+            self.model.drop_hoisted([i for st in finished for i in st.inputs()], keep)
         return done
 
-    def _run(self, states, forwards, scales, restored):
+    def _run(self, states, forwards, scales, flags):
         """The forwards of a tick, with the model's hoisted-tensor cache bounds raised as far as the live set needs
         and, if shared, the engine's graph pool; concatenations of chunks this tick did not use are dropped."""
         model = self.model
-        n_inputs = sum(len(_inputs_of(st.req)) + 1 for st in states)
-        bounds = {"hoist_cache_entries": n_inputs + 8,
-                  "cat_cache_entries": len(model._cat_cache) + len(forwards) + 1}
-        if self.share_graph_pool:
-            if self._pool is None:
-                self._pool = torch.cuda.graph_pool_handle()
-            bounds["graph_pool"] = self._pool
-        saved = {k: model.__dict__[k] for k in bounds if k in model.__dict__}
-        for k, v in bounds.items():
-            setattr(model, k, v if k == "graph_pool" else max(v, getattr(model, k, 0)))
+        if self.share_graph_pool and self._pool is None:
+            self._pool = torch.cuda.graph_pool_handle()
         n_graphs = len(model._graphs)
-        try:
-            evals = _evaluate(model, states, forwards, scales, restored, [e.null_input for e in self._live],
-                              per_image_conv=True)
-        finally:
-            for k in bounds:
-                if k in saved:
-                    setattr(model, k, saved[k])
-                else:
-                    delattr(model, k)
+        with _RequestState.cache_bounds(model, sum(st.plan.trajectories + 1 for st in states) + 8,
+                                        len(model._cat_cache) + len(forwards) + 1, self._pool):
+            evals = _RequestState.evaluate(model, states, forwards, scales, flags, per_image_conv=True)
         self.graphs_captured += len(model._graphs) - n_graphs
         model.trim_concats(len(forwards))
         self.forwards += len(forwards)

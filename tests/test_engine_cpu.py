@@ -1,34 +1,18 @@
 """Host logic of the continuous-batching engine (instancediffusion_b200.ldm.models.diffusion.engine): admission, the
 tick in which each evaluation, merge and finish happens, bucket padding, grouping by latent size, and the validation
-of `submit`.  Driven by a fake model whose eps is a function of its inputs, with the two sampler kernels restated in
-torch for the test, so no GPU is needed; each request's latent is compared with its own sampler run on the same fake."""
+of `submit`.  Driven by the fake model of fake_unet.py, so no GPU is needed; each request's latent is compared with its
+own sampler run on the same fake."""
 import os
 import sys
-from functools import partial
 
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from fake_unet import FakeUNet, _alone, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
 from instancediffusion_b200 import ops  # noqa: E402
-from instancediffusion_b200.ldm.models.diffusion.batched import Request, RequestPlan, schedule_steps  # noqa: E402
+from instancediffusion_b200.ldm.models.diffusion.batched import RequestPlan, schedule_steps  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion.engine import SamplingEngine, pick_bucket, plan_forwards  # noqa: E402
-from instancediffusion_b200.utils.model import alpha_generator  # noqa: E402
-
-
-def _plms_update(x, e_c, e_u, gs, olds, coefs, a_t, a_prev, s1m, e_out, x_out):
-    e = e_c if e_u is None else e_u + gs * (e_c - e_u)
-    ep = coefs[0] * e + sum(c * o for c, o in zip(coefs[1:], olds))
-    xp = a_prev ** 0.5 * (x - s1m * ep) / a_t ** 0.5 + (1 - a_prev) ** 0.5 * ep
-    if e_out is not None:
-        e_out.copy_(e)
-    x_out.copy_(xp)
-
-
-def _latent_mean(xs, out):
-    return out.copy_(torch.stack(xs).mean(0))
 
 
 @pytest.fixture(autouse=True)
@@ -37,76 +21,10 @@ def torch_kernels(monkeypatch):
     monkeypatch.setattr(ops, "latent_mean", _latent_mean)
 
 
-class FakeUNet(torch.nn.Module):
-    """eps depends on the latent, the timestep, the context, the fuser scale and the first conv of each image."""
-
-    def __init__(self):
-        super().__init__()
-        self.alpha, self._first_conv_restored = 0.0, False  # (a model without fusers runs at scale 0)
-        self._graphs, self._cat_cache = {}, {}
-        self.calls, self.dropped = [], []
-
-    def restore_first_conv_from_SD(self):
-        self._first_conv_restored = True
-
-    def forward_batched(self, inputs, *, scales=None, restored=None, per_image_conv=False):
-        n = len(inputs)
-        scales = [self.alpha] * n if scales is None else scales
-        restored = [self._first_conv_restored] * n if restored is None else restored
-        self.calls.append(dict(sizes=[i["x"].shape[0] for i in inputs], hw=[tuple(i["x"].shape[2:]) for i in inputs],
-                               t=[int(i["timesteps"].reshape(-1)[0]) for i in inputs], scales=list(scales),
-                               restored=list(restored), zero=[bool((i["x"] == 0).all()) for i in inputs]))
-        return [0.1 * i["x"] + 1e-4 * i["timesteps"].float().view(-1, 1, 1, 1) + 0.01 * i["context"].mean()
-                + 0.02 * s + 0.03 * float(r) for i, s, r in zip(inputs, scales, restored)]
-
-    def drop_hoisted(self, inputs, keep=()):
-        self.dropped.append(([id(i["context"]) for i in inputs], [id(i["context"]) for i in keep]))
-
-    def trim_concats(self, keep):
-        pass
-
-
 @pytest.fixture
 def diffusion():
     from instancediffusion_b200.ldm.models.diffusion.ldm import LatentDiffusion
     return LatentDiffusion(linear_start=0.00085, linear_end=0.012, timesteps=1000)
-
-
-AGEN = partial(alpha_generator, type=[0.8, 0.0, 0.2])
-
-
-def _req(seed, S, n=0, mis=0.0, size=64, ctx=77, alpha=AGEN, **kw):
-    g = torch.Generator().manual_seed(seed)
-    x = torch.randn((1, 4, size, size), generator=g)
-
-    def inp():
-        return dict(x=x, timesteps=None, context=torch.randn((1, ctx, 8), generator=g))
-    ins = [inp() for _ in range(n + 1)] if n else inp()
-    return Request(input=ins, uc=torch.zeros((1, ctx, 8)), guidance_scale=7.5, alpha_generator_func=alpha, mis=mis, S=S,
-                   **kw)
-
-
-def _fresh(req):
-    from dataclasses import replace
-    if isinstance(req.input, list):
-        x = req.input[0]["x"].clone()
-        return replace(req, input=[dict(i, x=x) for i in req.input])
-    return replace(req, input=dict(req.input, x=req.input["x"].clone()))
-
-
-def _alone(diffusion, req):
-    from instancediffusion_b200.ldm.models.diffusion.plms import PLMSSampler
-    from instancediffusion_b200.ldm.models.diffusion.plms_instance import PLMSSamplerInst
-    model = FakeUNet()
-    req = _fresh(req)
-    kw = dict(alpha_generator_func=req.alpha_generator_func, set_alpha_scale=lambda m, a: setattr(m, "alpha", a))
-    if isinstance(req.input, list):
-        s = PLMSSamplerInst(diffusion, model, mis=req.mis, **kw)
-    else:
-        s = PLMSSampler(diffusion, model, **kw)
-    return s.sample(S=req.S, shape=(1, 4) + tuple(req.input[0]["x"].shape[2:] if isinstance(req.input, list)
-                                                 else req.input["x"].shape[2:]), input=req.input, uc=req.uc,
-                    guidance_scale=req.guidance_scale)
 
 
 def _run(engine, arrivals):
@@ -229,5 +147,10 @@ def test_submit_validation(diffusion):
     with pytest.raises(ValueError, match="max_live_images"):
         eng.submit(_req(20, 10, n=4, mis=0.36))  # 5 trajectories x 2 images
     assert eng.queued == []
+    uneven = FakeUNet()
+    uneven.fusers[1].scale = 0.25
+    with pytest.raises(ValueError, match="differs between fusers"):
+        SamplingEngine(uneven, diffusion).submit(_req(20, 10, alpha=None))
+    SamplingEngine(uneven, diffusion).submit(_req(20, 10))  # a request with an alpha schedule sets its own scale
     with pytest.raises(ValueError, match="max_batch"):
         SamplingEngine(model, diffusion, max_batch=0)

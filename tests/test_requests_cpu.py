@@ -1,16 +1,21 @@
 """Host logic of the batched request sampler (instancediffusion_b200.ldm.models.diffusion.batched): the step planner
-that builds each step's forward chunks, and the validation of a request list.  No GPU needed."""
+that builds each step's forward chunks, the validation of a request list, and whole `sample_requests` runs on the fake
+model of fake_unet.py.  No GPU needed."""
 import os
 import sys
+from functools import partial
 
+import numpy as np
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from fake_unet import AGEN, FakeUNet, _alone, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
+from instancediffusion_b200 import ops  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion.batched import (  # noqa: E402
-    Request, RequestPlan, check_requests, plan_chunks, plan_step)
+    Request, RequestPlan, check_requests, plan_chunks, plan_step, sample_requests, schedule_steps)
+from instancediffusion_b200.ldm.modules.diffusionmodules.util import make_ddim_timesteps  # noqa: E402
+from instancediffusion_b200.utils.model import alpha_generator  # noqa: E402
 
 
 def _inp(b=1, size=64, ctx=77):
@@ -49,7 +54,6 @@ def test_trajectory_counts_and_merge_steps():
 def test_merge_step_follows_the_schedule_length():
     """The PLMS schedule of S steps is range(0, 1000, 1000 // S): 31 steps for S = 30, 12 for S = 11.  The merge comes
     before step int(len * mis), as PLMSSamplerInst computes it, and mis = 1 merges after the last step."""
-    from instancediffusion_b200.ldm.models.diffusion.batched import schedule_steps
     assert [schedule_steps(S) for S in (10, 11, 30, 50, 60)] == [10, 12, 31, 50, 63]
     assert check_requests([_mis_request(2)], 30, 32)[0].merge_step == 11   # not int(30 * 0.36) = 10
     assert check_requests([_mis_request(2)], 11, 32)[0].merge_step == 4    # not 3
@@ -98,3 +102,42 @@ def test_validation_errors():
     plans = check_requests([Request(input=dict(x=None, timesteps=None, context=torch.zeros((2, 77, 768))),
                                     shape=(2, 4, 64, 64))], 10, 32)
     assert plans[0].images == 2
+
+
+@pytest.mark.parametrize("S", [10, 11])
+def test_sample_requests_forwards_and_latents(monkeypatch, S):
+    """Plain, mis 0.36, mis 1.0 and no-alpha-schedule requests in one run on the fake UNet, its fusers at 0.5: every
+    forward (images, timesteps, fuser scales and conv flags per input, the corrector forwards of step 0 after the
+    predictor's), the model's conv and fuser scale afterwards, and each latent against the request's own sampler."""
+    from instancediffusion_b200.ldm.models.diffusion.ldm import LatentDiffusion
+    monkeypatch.setattr(ops, "plms_update", _plms_update)
+    monkeypatch.setattr(ops, "latent_mean", _latent_mean)
+    diffusion = LatentDiffusion(linear_start=0.00085, linear_end=0.012, timesteps=1000)
+    ones = partial(alpha_generator, type=[1.0, 0.0, 0.0])
+    reqs = [_req(31, S), _req(32, S, n=2, mis=0.36), _req(33, S, n=1, mis=1.0, alpha=ones), _req(34, S, alpha=None)]
+    model = FakeUNet(scale=0.5)
+    got = sample_requests(model, diffusion, [_fresh(r) for r in reqs], S, max_batch=8)
+    # a sequential run leaves the SD1.5 conv of the first two requests and the last alpha of the last alpha schedule
+    assert model._first_conv_restored and [f.scale for f in model.fusers] == [1.0, 1.0]
+
+    steps = schedule_steps(S)
+    t = [int(v) for v in np.flip(make_ddim_timesteps("uniform", S, 1000))]
+    alphas = [AGEN(steps), AGEN(steps), ones(steps), None]
+    plans = check_requests(reqs, S, 8)
+    want = []
+    for i in range(steps):
+        scale = [0.5 if a is None else float(a[i]) for a in alphas]
+        sd_conv = [a is not None and 0 in a[:i + 1] for a in alphas]  # from a request's first alpha-0 step on
+        for ts in ([t[0], t[1]] if i == 0 else [t[i]]):
+            for chunk in plan_step(plans, i, 8):
+                rows = [r for r, _ in chunk for _ in ("cond", "uncond")]
+                want.append(dict(sizes=[1] * len(rows), t=[ts] * len(rows), scales=[scale[r] for r in rows],
+                                 restored=[sd_conv[r] for r in rows]))
+    assert [{k: c[k] for k in want[0]} for c in model.calls] == want
+    for k, r in enumerate(reqs):
+        assert torch.allclose(got[k], _alone(diffusion, r, scale=0.5), rtol=1e-5, atol=1e-6), k
+
+    model = FakeUNet(scale=0.5)
+    model.fusers[1].scale = 0.25
+    with pytest.raises(ValueError, match="differs between fusers"):
+        sample_requests(model, diffusion, [_fresh(r) for r in reqs], S)
