@@ -38,6 +38,15 @@ int idiff_version(void);
 #define IDIFF_DTYPE_BF16 1
 int idiff_storage_dtype(void);
 
+/* Batch-invariant mode (process-wide, per library build; off by default).  While it is on, every image's
+ * output of every entry point below is a function of that image's inputs and the weights only: launch
+ * geometry that shapes a reduction depends on the per-image shape, never on the batch size, the total row
+ * count or the SM count.  In particular idiff_gemm runs data-parallel (no stream-K) with a tile width that
+ * depends on N and the epilogue family only, LayerNorm statistics (ln_stats_out) are taken over the stored
+ * 16-bit values, and GroupNorm / ScaleU reduce in a fixed number of pixel chunks per image.  Returns the
+ * previous setting. */
+int idiff_set_batch_invariant(int on);
+
 /* ---------------------------------------------------------------------------------------------
  * idiff_gemm: out = epilogue(A . W^T) on wgmma tensor cores (TMA-staged 128B-swizzled tiles,
  * fp32 accumulation in registers).  Replaces every nn.Linear / 1x1 conv / 3x3 conv of the path:

@@ -58,6 +58,7 @@ SIGNATURES = {
     "idiff_last_error": (C.c_char_p, []),
     "idiff_version": (_i, []),
     "idiff_storage_dtype": (_i, []),
+    "idiff_set_batch_invariant": (_i, [_i]),
     "idiff_gemm": (_i, [C.POINTER(GemmArgs), _vp]),
     "idiff_gemm_ln_slots": (_i, [C.POINTER(GemmArgs)]),
     "idiff_row_stats": (_i, [_vp, _vp, _i, _i, _vp]),
@@ -95,6 +96,15 @@ SIGNATURES = {
 
 _libs = {}
 _storage = "f16"  # which build load() returns; switched by ops.set_storage_dtype
+_batch_invariant = False  # idiff_set_batch_invariant of every loaded build; switched by ops.set_batch_invariant
+
+
+def set_batch_invariant(on: bool) -> None:
+    """Set the mode in every build loaded so far; load() sets it in builds loaded later."""
+    global _batch_invariant
+    _batch_invariant = bool(on)
+    for lib in _libs.values():
+        lib.idiff_set_batch_invariant(int(_batch_invariant))
 
 
 def set_storage(kind: str) -> None:
@@ -127,6 +137,7 @@ def load(kind: str | None = None) -> C.CDLL:
         fn.argtypes = args
     if lib.idiff_storage_dtype() != DTYPE_CODES[kind]:
         raise IdiffError(f"{path} was not built for {kind} storage")
+    lib.idiff_set_batch_invariant(int(_batch_invariant))
     _libs[kind] = lib
     return lib
 

@@ -150,7 +150,8 @@ IDIFF_DEVICE uint32_t epi_offset(int row, int jj) {
   return (uint32_t)((jj >> 2) * EPI_SLAB_BYTES + row * 64 + (((jj & 3) ^ ((row >> 1) & 3)) << 4));
 }
 
-template <int BN, int MODE>
+// LNR: producer LayerNorm statistics of the stored 16-bit values instead of the fp32 results (batch-invariant mode)
+template <int BN, int MODE, bool LNR = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR, const Params p) {
@@ -561,6 +562,13 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
                 x0 = fmaf(g, x0, r.x);
                 x1 = fmaf(g, x1, r.y);
               }
+              if constexpr (LNR) {
+                // the stored values: a row that a gate of 0 passes through unchanged keeps the statistics its
+                // producer wrote, so skipping a fuser and gating it off agree bit for bit
+                const float2 y = unpack_half2(pack_half2(x0, x1));
+                x0 = y.x;
+                x1 = y.y;
+              }
               if (lno && cok) {
                 ln_ps[hh] += x0 + x1;
                 ln_pq[hh] = fmaf(x0, x0, fmaf(x1, x1, ln_pq[hh]));
@@ -634,7 +642,7 @@ static int encode_epi_map(CUtensorMap* m, const void* base, int n, int ld, const
   return encode_tmap_f16_sw(m, base, 2, dims, strides, box, 64);
 }
 
-template <int BN, int MODE>
+template <int BN, int MODE, bool LNR = false>
 static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
   using C = Cfg<BN, MODE>;
   Params p;
@@ -719,7 +727,7 @@ static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
   void* ws_ptr = a->workspace ? a->workspace : g_ws;
   const long ws_bytes = a->workspace ? a->workspace_bytes : g_ws_bytes;
   const int workers = g_num_sms;
-  const bool use_sk = want_sk && ws_ptr && ws_bytes >= ws_need && p.KB >= 8 && (p.T % g_num_sms) != 0 &&
+  const bool use_sk = want_sk && !batch_invariant() && ws_ptr && ws_bytes >= ws_need && p.KB >= 8 && (p.T % g_num_sms) != 0 &&
                       (long)p.T * p.KB >= g_num_sms;
   if (use_sk) {
     p.G = g_num_sms;
@@ -736,11 +744,11 @@ static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
 
   static bool attr_set = false;
   if (!attr_set) {
-    IDIFF_CHECK_CUDA(cudaFuncSetAttribute(gemm2_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    IDIFF_CHECK_CUDA(cudaFuncSetAttribute(gemm2_kernel<BN, MODE, LNR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           C::SMEM_BYTES));
     attr_set = true;
   }
-  IDIFF_CHECK_CUDA(launch_pdl(gemm2_kernel<BN, MODE>, dim3(p.G), dim3(THREADS), C::SMEM_BYTES, stream, tmA, tmB, tmO, tmR, p));
+  IDIFF_CHECK_CUDA(launch_pdl(gemm2_kernel<BN, MODE, LNR>, dim3(p.G), dim3(THREADS), C::SMEM_BYTES, stream, tmA, tmB, tmO, tmR, p));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -785,6 +793,7 @@ static Plan plan_gemm(const idiff_gemm_args* a, int fixed_bn, int max_bn = 256) 
   }
   Plan best = {fixed_bn ? fixed_bn : 128, false};
   double best_cost = -1;
+  const bool invariant = batch_invariant();
   for (int i = 0; i < 4; ++i) {
     const int bn = cands[i];
     if ((fixed_bn && bn != fixed_bn) || bn > max_bn) continue;
@@ -793,6 +802,16 @@ static Plan plan_gemm(const idiff_gemm_args* a, int fixed_bn, int max_bn = 256) 
     if (!fixed_bn && pad > min_pad + min_pad / 14) continue;  // more than ~7 % wasted columns
     const long T = (long)((a->N + bn - 1) / bn) * m_tiles;
     const double t_kb = fmax(2.0 * bn, (16384.0 + 128.0 * bn) / 80.0);
+    if (invariant) {
+      // batch-invariant mode: data-parallel, and the tile width from N alone -- the one with the least k-block
+      // time per row over all its column tiles, which is what the data-parallel cost tends to at large M
+      const double cost = (double)((a->N + bn - 1) / bn) * t_kb;
+      if (best_cost < 0 || cost < best_cost) {
+        best_cost = cost;
+        best = {bn, false};
+      }
+      continue;
+    }
     const double t_epi = 1500.0 * bn / 32.0;
     const double t_tile = KB * t_kb + 600.0;
     const long rounds = (T + sms - 1) / sms;
@@ -814,7 +833,7 @@ static Plan plan_gemm(const idiff_gemm_args* a, int fixed_bn, int max_bn = 256) 
       }
     }
   }
-  if (force) {
+  if (force && !invariant) {  // (the override would bring back stream-K and batch-dependent tile widths)
     int fbn = 0, fsk = 0;
     if (sscanf(force, "%d,%d", &fbn, &fsk) == 2) {
       if (!fixed_bn && fbn <= max_bn && (fbn == 256 || fbn == 192 || fbn == 160 || fbn == 128)) best.bn = fbn;
@@ -829,7 +848,8 @@ struct Resolved {
   bool sk;
 };
 
-static Resolved resolve(const idiff_gemm_args* a) {
+// stats: the launch writes LayerNorm statistics (ln_stats_out)
+static Resolved resolve(const idiff_gemm_args* a, bool stats) {
   // GEGLU: one 256-column accumulator tile = 128 value columns + their 128 gates (packing.py)
   if (a->flags & IDIFF_EPI_GEGLU) return {256, MODE_GEGLU, plan_gemm(a, 256).sk};
   if (a->flags & IDIFF_OUT_F32_NCHW) return {128, MODE_NCHW, plan_gemm(a, 128).sk};
@@ -838,12 +858,24 @@ static Resolved resolve(const idiff_gemm_args* a) {
     const Plan pl = plan_gemm(a, 0, 192);
     return {pl.bn, MODE_GATED, pl.sk};
   }
-  const Plan pl = plan_gemm(a, 0);
+  // Batch-invariant mode: plain producers of LayerNorm statistics share the gated cap, so a fuser that runs
+  // per-image gated and one that is skipped (its stream's statistics then come from the plain GEMM before it)
+  // hand the next LayerNorm the same slot partition.
+  const Plan pl = plan_gemm(a, 0, batch_invariant() && stats ? 192 : 256);
   return {pl.bn, MODE_PLAIN, pl.sk};
 }
 
 template <int MODE>
 static int launch_bn(const idiff_gemm_args* a, cudaStream_t stream, const Resolved& r) {
+  // batch-invariant producers of LayerNorm statistics (resolve caps them at 192)
+  if (batch_invariant() && a->ln_stats_out) {
+    switch (r.bn) {
+      case 192: return launch<192, MODE, true>(a, stream, r.sk);
+      case 160: return launch<160, MODE, true>(a, stream, r.sk);
+      case 128: return launch<128, MODE, true>(a, stream, r.sk);
+      default: return set_error("idiff_gemm: no stored-statistics kernel of tile width %d (resolve caps them at 192)", r.bn);
+    }
+  }
   switch (r.bn) {
     case 256:
       if constexpr (MODE != MODE_GATED) return launch<256, MODE>(a, stream, r.sk);
@@ -856,7 +888,7 @@ static int launch_bn(const idiff_gemm_args* a, cudaStream_t stream, const Resolv
 
 // One instantiation per (tile width, epilogue mode): each kernel carries only its own mode's code.
 int gemm_v2(const idiff_gemm_args* a, cudaStream_t stream) {
-  const Resolved r = resolve(a);
+  const Resolved r = resolve(a, a->ln_stats_out != nullptr);
   if (r.mode == MODE_GEGLU) return launch<256, MODE_GEGLU>(a, stream, r.sk);
   if (r.mode == MODE_NCHW) return launch<128, MODE_NCHW>(a, stream, r.sk);
   if (r.mode == MODE_GATED) return launch_bn<MODE_GATED>(a, stream, r);
@@ -865,7 +897,7 @@ int gemm_v2(const idiff_gemm_args* a, cudaStream_t stream) {
 
 // slots of the LayerNorm partial statistics a producer GEMM with these arguments writes per row
 int ln_slots_of(const idiff_gemm_args* a) {
-  const Resolved r = resolve(a);
+  const Resolved r = resolve(a, true);
   return (a->N + r.bn - 1) / r.bn;
 }
 

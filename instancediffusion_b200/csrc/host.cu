@@ -96,7 +96,17 @@ int num_sms() {
   return n;
 }
 
+static int g_batch_invariant = 0;
+
+bool batch_invariant() { return g_batch_invariant != 0; }
+
 }  // namespace idiff
+
+extern "C" int idiff_set_batch_invariant(int on) {
+  const int prev = idiff::g_batch_invariant;
+  idiff::g_batch_invariant = on ? 1 : 0;
+  return prev;
+}
 
 extern "C" const char* idiff_last_error(void) { return idiff::g_err; }
 extern "C" int idiff_version(void) { return 2; }

@@ -45,6 +45,16 @@ int encode_tmap_f16_sw(CUtensorMap* map, const void* base, int rank, const uint6
 bool pdl_enabled();
 // multiprocessor count of the current device (queried once; grid sizes of the bandwidth-bound kernels)
 int num_sms();
+// idiff_set_batch_invariant: reduction geometry must not depend on the batch, M or num_sms()
+bool batch_invariant();
+// Pixel chunks per image of a batch-invariant GroupNorm / ScaleU reduction over hw x channels: about 8K elements
+// (16 KB of 16-bit storage) per CTA, 1..max_chunks -- from the per-image shape alone.  At the UNet's 64x64 levels
+// this is the cap, as the batch-dependent rule gives up to batch 8; at 8x8 x 1280 it is 10 chunks instead of 1-pixel
+// ones; a VAE plane gets the cap.
+inline int invariant_chunks(int hw, int channels, int max_chunks) {
+  const long c = ((long)hw * channels + 8191) / 8192;
+  return c < 1 ? 1 : c > max_chunks ? max_chunks : (int)c;
+}
 template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
                        Args&&... args) {

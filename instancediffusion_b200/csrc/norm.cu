@@ -536,8 +536,10 @@ static void gn_geometry(int batch, int hw, int channels, int* k, int* ppb, int* 
   int kk = 256 / CV;
   if (kk < 1) kk = 1;
   if (kk > hw) kk = hw;
-  // aim at >= ~4 CTAs per SM over the whole launch, at most GN_MAX_CHUNKS chunks per sample
-  int want = (idiff::num_sms() * 4 + batch - 1) / batch;
+  // aim at >= ~4 CTAs per SM over the whole launch, at most GN_MAX_CHUNKS chunks per sample; batch-invariant
+  // mode: a count from the per-image shape (invariant_chunks)
+  int want = idiff::batch_invariant() ? idiff::invariant_chunks(hw, channels, idiff::GN_MAX_CHUNKS)
+                                      : (idiff::num_sms() * 4 + batch - 1) / batch;
   if (want > idiff::GN_MAX_CHUNKS) want = idiff::GN_MAX_CHUNKS;
   if (want < 1) want = 1;
   int p = (hw + want - 1) / want;
@@ -591,7 +593,8 @@ extern "C" int idiff_groupnorm(const void* x, void* y, const float* gamma, const
     // Single-pass cluster kernel wherever the launch fits one wave (gn_fused_geometry);
     // IDIFF_GN_FUSED=0 forces the two-kernel path (read per call so tests can cover both).
     const char* fe = getenv("IDIFF_GN_FUSED");
-    const bool fused_on = !(fe && fe[0] == '0');
+    // (batch-invariant mode: the single pass's cluster size follows the batch, so the two-kernel path runs)
+    const bool fused_on = !(fe && fe[0] == '0') && !batch_invariant();
     int CS, CL, kf;
     size_t smem_f;
     if (fused_on && gn_fused_geometry(batch, hw, channels, groups, &CS, &CL, &kf, &smem_f)) {

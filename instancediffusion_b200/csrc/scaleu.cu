@@ -180,11 +180,12 @@ scaleu_apply_kernel(const uint4* __restrict__ h, const uint4* __restrict__ skip,
   }
 }
 
-static void su_geometry(int batch, int hw, int cv, int max_chunks, int* k, int* ppb, int* chunks) {
+// invariant: the pass reduces over the chunks (the coefficients), so batch-invariant mode fixes their count per image
+static void su_geometry(int batch, int hw, int cv, int max_chunks, bool invariant, int* k, int* ppb, int* chunks) {
   int kk = 256 / cv;  // (512-thread CTAs with half as many chunks measured slower, like the GroupNorm passes)
   if (kk < 1) kk = 1;
   if (kk > hw) kk = hw;
-  int want = (num_sms() * 3 + batch - 1) / batch;
+  int want = invariant ? invariant_chunks(hw, cv * 8, max_chunks) : (num_sms() * 3 + batch - 1) / batch;
   if (want > max_chunks) want = max_chunks;
   if (want < 1) want = 1;
   int p = (hw + want - 1) / want;
@@ -212,7 +213,7 @@ extern "C" int idiff_scaleu_concat(const void* h, const void* skip, void* out, c
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int hw = height * width;
   int k1, ppb1, chunks1;
-  su_geometry(batch, hw, c2 / 8, SU_MAX_CHUNKS, &k1, &ppb1, &chunks1);
+  su_geometry(batch, hw, c2 / 8, SU_MAX_CHUNKS, batch_invariant(), &k1, &ppb1, &chunks1);
   const size_t smem = (size_t)k1 * c2 * 7 * sizeof(float);
   static bool attr_set = false;
   if (!attr_set) {
@@ -224,7 +225,7 @@ extern "C" int idiff_scaleu_concat(const void* h, const void* skip, void* out, c
   float* coef = coef_ws + (long)batch * SU_MAX_CHUNKS * c2 * 8;
   IDIFF_CHECK_CUDA(launch_pdl(scaleu_reduce_kernel, dim3((batch * c2 * 8 + 255) / 256), dim3(256), 0, st, coef_ws, coef, chunks1, c2, batch));
   int k2, ppb2, chunks2;
-  su_geometry(batch, hw, (c1 + c2) / 8, 4096, &k2, &ppb2, &chunks2);
+  su_geometry(batch, hw, (c1 + c2) / 8, 4096, false, &k2, &ppb2, &chunks2);  // (per-pixel: any chunking)
   IDIFF_CHECK_CUDA(launch_pdl(scaleu_apply_kernel, dim3(dim3(chunks2, batch)), dim3(k2 * ((c1 + c2) / 8)), 0, st,  reinterpret_cast<const uint4*>(h), reinterpret_cast<const uint4*>(skip), reinterpret_cast<uint4*>(out), b1, coef, s - 1.0f, height, width, c1, c2, ppb2, k2, 1));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;

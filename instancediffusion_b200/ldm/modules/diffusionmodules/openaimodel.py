@@ -739,21 +739,33 @@ class UNetModel(PackedModule):
 
         scales: one fuser scale per input -- what set_alpha_scale would set for a forward of that input alone --
         instead of the fusers' own `.scale`.  Equal scales run the scalar-gate path (all 0: the fusers are skipped);
-        mixed scales run the fusers on every image with the gates tanh(alpha) * scale of each image.
+        mixed scales run the fusers on every image with the gates tanh(alpha) * scale of each image.  In batch-invariant
+        mode (ops.set_batch_invariant) any non-zero scale takes the per-image gates, and every input conv is per image
+        as with per_image_conv.
         restored: per input, True = the SD1.5 input conv that restore_first_conv_from_SD swaps in, False = the
         model's own; the model's conv is not swapped.  Default: the model's current first-conv state.
         per_image_conv: choose each image's input conv on the device (ops.conv_in_select) from a per-image flag that,
         like the per-image scales, is a static input of the captured graph.  The count of SD1.5-conv images then
         stays out of the graph key, and the images keep their order."""
-        if getattr(self, "_storage_epoch", None) != ops.STORAGE_EPOCH:  # storage type switched: derived tensors are stale
+        # storage type or batch-invariant mode switched: derived tensors and captured graphs are stale
+        if getattr(self, "_storage_epoch", None) != (ops.STORAGE_EPOCH, ops.MODE_EPOCH):
             self._drop_derived()
-            self._storage_epoch = ops.STORAGE_EPOCH
+            self._storage_epoch = (ops.STORAGE_EPOCH, ops.MODE_EPOCH)
         n = len(inputs)
         for arg, name in ((scales, "scales"), (restored, "restored")):
             if arg is not None and len(arg) != n:
                 raise ValueError(f"forward_batched: {len(arg)} {name} for {n} inputs")
         sizes = [inp["x"].shape[0] for inp in inputs]
-        if per_image_conv:
+        # batch-invariant mode: one arithmetic path per image whatever the call -- every input conv runs per image
+        # (ops.conv_in_select), and fusers run with per-image gates unless every image skips them
+        invariant = ops.batch_invariant()
+        if invariant and scales is None:
+            own = {float(blk.fuser.scale) for st in self._transformers() for blk in st.transformer_blocks}
+            if len(own) != 1:  # (set_alpha_scale sets them all alike; only the scalar path could serve this)
+                raise ValueError(f"forward_batched: batch-invariant mode needs one fuser scale for the model, the "
+                                 f"fusers have {sorted(own)}; pass scales= instead")
+            scales = [own.pop()] * n
+        if per_image_conv or invariant:
             order = list(range(n))
             cur = bool(getattr(self, "_first_conv_restored", False))
             flags = [bool(restored[i]) if restored is not None else cur for i in range(n)]
@@ -771,7 +783,7 @@ class UNetModel(PackedModule):
         fuser_scale, active = None, None
         if scales is not None:
             s = [float(scales[i]) for i in order]
-            if all(v == s[0] for v in s):
+            if all(v == s[0] for v in s) and not (invariant and s[0] != 0):
                 fuser_scale, active = s[0], s[0] != 0
             else:
                 rows = torch.tensor([v for v, i in zip(s, order) for _ in range(sizes[i])], dtype=torch.float32)

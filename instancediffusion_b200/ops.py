@@ -39,6 +39,27 @@ def storage_dtype() -> torch.dtype:
     return HALF
 
 
+# Batch-invariant mode (include/idiff_b200.h idiff_set_batch_invariant): every image's result depends on that image's
+# inputs and the weights only, not on what else is in the batch.  Off by default.
+BATCH_INVARIANT = False
+MODE_EPOCH = 0  # bumped on every switch: hoisted tensors and graphs computed in the other mode are stale
+
+
+def set_batch_invariant(on: bool) -> None:
+    """Turn batch-invariant mode on or off for every kernel launched afterwards.  The UNet drops its hoisted tensors
+    and captured graphs on next use, so nothing computed in the other mode is replayed."""
+    global BATCH_INVARIANT, MODE_EPOCH
+    on = bool(on)
+    if on != BATCH_INVARIANT:
+        _lib.set_batch_invariant(on)
+        BATCH_INVARIANT = on
+        MODE_EPOCH += 1
+
+
+def batch_invariant() -> bool:
+    return BATCH_INVARIANT
+
+
 class storage:
     """Context manager: `with ops.storage(torch.bfloat16): ...`."""
 

@@ -3,7 +3,10 @@ images at 512^2).  Each shape: 3 warm-ups, then N timed launches bracketed by CU
 launching stream with an L2 flush (256 MB write) between launches.  Prints one table row per shape
 and a JSON blob (gpurun_out/kernels_<tag>.json).
 
-  python tools/bench_kernels.py [tag] [gemm|attn|norm|all]
+  python tools/bench_kernels.py [tag] [gemm|attn|norm|all] [--batch N] [--batch-invariant]
+
+--batch-invariant runs every kernel in batch-invariant mode (ops.set_batch_invariant), so per-shape costs of the
+two modes can be compared; --batch sets the forward batch (default 8).
 """
 import json
 import math
@@ -17,10 +20,16 @@ from instancediffusion_b200 import ops  # noqa: E402
 from instancediffusion_b200.packing import pack_geglu  # noqa: E402
 
 dev = torch.device("cuda:0")
-tag = sys.argv[1] if len(sys.argv) > 1 else "run"
-which = sys.argv[2] if len(sys.argv) > 2 else "all"
-flush = torch.zeros(64 << 20, dtype=torch.int32, device=dev)  # 256 MB, read to evict L2 with clean lines
+argv = [a for a in sys.argv[1:] if a != "--batch-invariant"]
 B = 8
+if "--batch" in argv:
+    i = argv.index("--batch")
+    B = int(argv[i + 1])
+    del argv[i:i + 2]
+tag = argv[0] if len(argv) > 0 else "run"
+which = argv[1] if len(argv) > 1 else "all"
+ops.set_batch_invariant("--batch-invariant" in sys.argv)
+flush = torch.zeros(64 << 20, dtype=torch.int32, device=dev)  # 256 MB, read to evict L2 with clean lines
 
 
 def timed(fn, iters=5):
@@ -139,12 +148,15 @@ if which in ("all", "attn"):
 
 if which in ("all", "norm"):
     print(f"\n{'norm / elementwise':30s} {'us':>8s} {'GB/s (4B/elt)':>14s}")
-    for hw, C in [(4096, 320), (4096, 640), (4096, 960), (1024, 640), (1024, 1280), (1024, 1920), (256, 1280), (256, 2560), (64, 1280), (64, 2560)]:
-        x = rnd(B * hw, C)
+    # UNet shapes, then VAE decoder planes (the two largest at one image: 512 MB per batch-8 tensor)
+    for hw, C in [(4096, 320), (4096, 640), (4096, 960), (1024, 640), (1024, 1280), (1024, 1920), (256, 1280), (256, 2560), (64, 1280), (64, 2560),
+                  (4096, 512), (16384, 512), (65536, 256), (262144, 128)]:
+        Bn = 1 if hw * C > (1 << 24) else B
+        x = rnd(Bn * hw, C)
         g = torch.ones(C, device=dev)
         bb = torch.zeros(C, device=dev)
         out = torch.empty_like(x)
-        t = timed(lambda: ops.groupnorm(x, g, bb, batch=B, hw=hw, silu=True, out=out))
+        t = timed(lambda: ops.groupnorm(x, g, bb, batch=Bn, hw=hw, silu=True, out=out))
         rows.append(dict(kind="groupnorm", label=f"gn {hw}x{C}", us=t * 1e6, gbs=4.0 * x.numel() / t / 1e9))
         print(f"{f'groupnorm {hw}x{C}':30s} {t * 1e6:8.1f} {4.0 * x.numel() / t / 1e9:14.0f}")
     for hw, C in [(4096, 320), (1024, 640), (256, 1280), (64, 1280)]:

@@ -41,6 +41,9 @@ def main():
     ap.add_argument("--requests", type=int, default=24)
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--load", default="0.5,1.0", help="arrival rate(s) as multiples of the single-request rate")
+    ap.add_argument("--base-rate", type=float, default=None,
+                    help="requests/s that --load multiplies instead of the measured single-request rate: the same "
+                         "arrival trace in runs that compare two builds or modes")
     ap.add_argument("--max-batch", type=int, default=32)
     ap.add_argument("--share-pool", action="store_true", help="the engine's graphs share one memory pool")
     ap.add_argument("--seed", type=int, default=0)
@@ -165,7 +168,8 @@ def main():
 
     result = {}
     for load in [float(v) for v in args.load.split(",")]:
-        gaps = np.random.default_rng(args.seed + 1).exponential(1.0 / (load * single_rate), len(base))
+        rate = args.base_rate if args.base_rate else single_rate
+        gaps = np.random.default_rng(args.seed + 1).exponential(1.0 / (load * rate), len(base))
         arrivals = np.cumsum(gaps) - gaps[0]
         per, outs = {}, {}
         for name, fn in arms.items():
@@ -188,7 +192,7 @@ def main():
         "workload": f"{len(base)} requests x 1 image 512x512, n={ns}, MIS 0.36 (every 6th plain PLMS), S={args.steps} "
                     f"(every 5th S={args.steps // 2}), CFG 7.5, alpha [0.8, 0, 0.2], Poisson arrivals, fp16",
         "gpu": gpu_info(), "max_batch": args.max_batch, "share_graph_pool": args.share_pool,
-        "single_request_rate_per_s": single_rate,
+        "single_request_rate_per_s": single_rate, "base_rate_per_s": args.base_rate,
         "engine_warmup": {**warm_engine, "max_memory_reserved_gib": engine_reserved / 2 ** 30},
         "graphs_total": len(model._graphs), "loads": result,
     }
