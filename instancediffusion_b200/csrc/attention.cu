@@ -1,13 +1,15 @@
 // Flash-style attention on wgmma for sm_90a: O = softmax(Q K^T * scale) V per (batch, head).
 //
-// One CTA owns a 128-query tile of one (batch, head): warpgroup 0 is the TMA producer (Q once, then
-// K / V tiles of 128 keys at d = 40, 64 keys otherwise, through a ring), warpgroups 1 and 2 each own
-// 64 query rows.  Per key block a consumer warpgroup computes S = Q K^T with wgmma (Q and K from
-// 128B-swizzled shared memory) into registers, runs the online softmax on the fragments (a row lives
-// in the four threads of a quad), and feeds P straight from registers as the A operand of O += P V
-// at N = d; V is consumed as an MN-major B operand from its token-major tile, so no transposed copy
-// of V is ever made.  The PV product of block j - 1 runs on the tensor cores during the softmax of
-// block j.  O stays in registers and is normalised and stored at the end.
+// One CTA owns a query tile of one (batch, head): warpgroup 0 is the TMA producer (Q once, then
+// K / V tiles of 128 keys at d = 40, 64 keys otherwise, through a ring), and each consumer warpgroup
+// owns 64 query rows: three of them (a 192-query tile) at d = 40, two (128 queries) otherwise.  Per key
+// block a consumer warpgroup computes S = Q K^T with wgmma (Q and K from 128B-swizzled shared memory)
+// into registers, runs the online softmax on the fragments (a row lives in the four threads of a quad),
+// and feeds P straight from registers as the A operand of O += P V at N = d; V is consumed as an
+// MN-major B operand from its token-major tile, so no transposed copy of V is ever made.  With two
+// consumer warpgroups the PV product of block j - 1 runs on the tensor cores during the softmax of
+// block j; with three, the other warpgroups' work fills that time.  O stays in registers and is
+// normalised and stored at the end.
 // Keys/values are read from up to two segments (visual tokens, then the 184 UniFusion object
 // tokens of GatedSelfAttentionDense) -- the concatenation of attention.py:306 never exists.
 // The optional instance-isolation mask (attention.py:187-255) is applied to the scores: query i may
@@ -21,9 +23,6 @@
 #include "wgmma.cuh"
 
 namespace idiff {
-
-constexpr int ATT_THREADS = 384;
-constexpr int BQ = 128;
 
 struct AttnKParams {
   int heads, nq, n0, n1, kv1_broadcast;
@@ -42,18 +41,34 @@ struct AttnCfg {
   // waits, wgmma issue and latency, row-max shuffles, O rescale); at d >= 80 S + P + O must fit in registers
   static constexpr int BKV = (D <= 64) ? 128 : 64;
   static constexpr int STAGES = (D <= 64) ? 4 : 3;
+  // consumer warpgroups of 64 query rows.  At d = 40 a row's softmax is a long dependent chain (max, subtract,
+  // exp2, row sum, pack) next to little tensor work, so a third warpgroup gives each scheduler another
+  // independent softmax warp to issue from; at d >= 80 the S + P + O fragments need 232 registers a thread.
+  static constexpr int NCW = (D <= 64) ? 3 : 2;
+  static constexpr int BQ = 64 * NCW;
+  static constexpr int THREADS = 128 * (NCW + 1);
+  // register split (setmaxnreg at the head of each role branch): 128 x PRODUCER + 128 NCW x CONSUMER <= 65536
+  static constexpr int PRODUCER_REGS = (NCW == 3) ? 24 : 40;
+  static constexpr int CONSUMER_REGS = (NCW == 3) ? 160 : 232;
+  static_assert(128 * PRODUCER_REGS + 128 * NCW * CONSUMER_REGS <= 65536, "register split");
+  // With two consumer warpgroups each one also keeps its own PV product of block j - 1 on the tensor cores while
+  // it runs the softmax of block j, which keeps P_{j-1} (BKV / 4 registers) live next to S_j.  ptxas allocates
+  // no thread more than the launch bound's 65536 / THREADS registers whatever setmaxnreg grants (128 at 512
+  // threads), and that loop needs about 140 at d = 40; with three warpgroups a consumer waits for its PV
+  // product before the softmax, and the other two warpgroups' wgmmas and softmaxes fill the wait.
+  static constexpr bool PV_UNDER_SOFTMAX = NCW == 2;
   static constexpr int Q_BYTES = ND * BQ * 128;
   static constexpr int KV_TILE_BYTES = ND * BKV * 128;  // one of K or V
   static constexpr int SMEM_BYTES = 1024 + Q_BYTES + STAGES * 2 * KV_TILE_BYTES + 256;  // + alignment slack, barriers
 };
 
 template <int D, bool MASKED>
-__global__ void __launch_bounds__(ATT_THREADS, 1)
+__global__ void __launch_bounds__(AttnCfg<D>::THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
                  const __grid_constant__ CUtensorMap tmV0, const __grid_constant__ CUtensorMap tmK1,
                  const __grid_constant__ CUtensorMap tmV1, const AttnKParams p) {
   using Cfg = AttnCfg<D>;
-  constexpr int ND = Cfg::ND, STAGES = Cfg::STAGES, BKV = Cfg::BKV;
+  constexpr int ND = Cfg::ND, STAGES = Cfg::STAGES, BKV = Cfg::BKV, NCW = Cfg::NCW, BQ = Cfg::BQ;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -83,7 +98,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&k_full[s], 1);
       mbar_init(&v_full[s], 1);
-      mbar_init(&kv_empty[s], 8);
+      mbar_init(&kv_empty[s], 4 * NCW);
     }
     fence_barrier_init();
   }
@@ -92,8 +107,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   pdl_wait();               // operands come from earlier kernels: nothing above touched global memory
 
   if (warp < 4) {
-    // register split: 40 x 128 + 232 x 256 <= the CTA's 65536 (setmaxnreg at the head of each role branch)
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(Cfg::PRODUCER_REGS));
     // ===================== TMA producer =====================
     if (threadIdx.x == 0) {
       mbar_expect_tx(q_full, Cfg::Q_BYTES);
@@ -119,14 +133,34 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       }
     }
   } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(Cfg::CONSUMER_REGS));
     // ===================== consumers: S = Q K^T, online softmax, O += P V =====================
     // Per key block j a consumer issues S_j = Q K_j^T and O += P_{j-1} V_{j-1} back to back, runs the
-    // softmax of S_j while the PV product is still on the tensor cores, then waits for it and rescales O.
-    // The two consumer warpgroups also take turns issuing (named barrier 1 + cw grants warpgroup cw its
-    // turn), so one warpgroup's softmax runs under the other's wgmmas.
+    // softmax of S_j while the PV product is still on the tensor cores, then waits for it and rescales O
+    // (PV_UNDER_SOFTMAX; otherwise PV_{j-1} retires before S_j is issued, and O is rescaled after the softmax).
+    // The consumer warpgroups also take turns issuing, round robin (named barrier 1 + cw grants warpgroup cw
+    // its turn; each turn grants the next warpgroup's), so one warpgroup's softmax runs under the others' wgmmas.
     const int cw = (warp >> 2) - 1;  // rows [64 cw, 64 cw + 64) of the query tile
-    const uint32_t my_turn = 1 + cw, their_turn = 2 - cw;
+    const uint32_t my_turn = 1 + cw, next_turn = 1 + (cw + 1) % NCW;
+    if (cw == NCW - 1) named_bar_arrive(1, 256);  // warpgroup 0 takes the first turn
+    if (q0 + cw * 64 >= p.nq) {
+      // every row of this warpgroup lies past nq (the last tile of a ragged nq): no math, but it still takes
+      // its T + 1 turns and releases each K/V stage once that stage's fill has landed, as the loop below does
+      uint32_t s = 0, ph = 0;
+      for (int j = 0; j <= T; ++j) {
+        named_bar_sync(my_turn, 256);
+        if (j < T || cw != NCW - 1) named_bar_arrive(next_turn, 256);
+        if (j < T) {
+          mbar_wait(&v_full[s], ph);
+          if (lane == 0) mbar_arrive(&kv_empty[s]);
+          if (++s == STAGES) {
+            s = 0;
+            ph ^= 1;
+          }
+        }
+      }
+      return;
+    }
     const int t4 = lane & 3;
     const int rl0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);  // tile rows of this thread: rl0, rl0 + 8
     const float c = p.scale_log2e;
@@ -253,13 +287,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         }
     };
 
-    // PV_{j-2} has retired: free its K/V stage, rescale O by the factor of block j - 1 and pack P_{j-1}.
-    // Called at the top of a trip, not after the softmax: the compiler must not hoist the wait into the
-    // softmax (where it would stall on the PV product the softmax is meant to hide).
-    auto retire_pv = [&](bool release, uint32_t st) {
-      wgmma_wait<0>();
-      wgmma_fence_regs(o);
-      if (release && lane == 0) mbar_arrive(&kv_empty[st]);
+    // rescale O by the factor of the block just through the softmax and pack its P
+    auto rescale_pack = [&]() {
       // alpha is exactly 1 where the row max did not move (most blocks once a row has seen a few):
       // skip the multiply when that holds for every row of the warp
       if (!__all_sync(0xffffffffu, alpha[0] == 1.f && alpha[1] == 1.f)) {
@@ -273,44 +302,71 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       }
       pack_p();
     };
+    // PV_{j-2} has retired: free its K/V stage, rescale O by the factor of block j - 1 and pack P_{j-1}.
+    // Called at the top of a trip, not after the softmax: the compiler must not hoist the wait into the
+    // softmax (where it would stall on the PV product the softmax is meant to hide).
+    auto retire_pv = [&](bool release, uint32_t st) {
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+      if (release && lane == 0) mbar_arrive(&kv_empty[st]);
+      rescale_pack();
+    };
 
     mbar_wait(q_full, 0);
-    if (cw == 1) named_bar_arrive(1, 256);  // warpgroup 0 takes the first turn
     named_bar_sync(my_turn, 256);
     mbar_wait(&k_full[0], 0);
     wgmma_fence();
     issue_qk(0);
-    named_bar_arrive(their_turn, 256);
+    named_bar_arrive(next_turn, 256);
     wgmma_wait<0>();
     wgmma_fence_regs(sc);
     softmax(0);
+    if (!Cfg::PV_UNDER_SOFTMAX) rescale_pack();
     uint32_t s = 0, ph = 0;  // ring stage / phase of block j - 1
     uint32_t s_prev = 0;     // ring stage of block j - 2
     for (int j = 1; j < T; ++j) {
-      retire_pv(j >= 2, s_prev);
+      if (Cfg::PV_UNDER_SOFTMAX) retire_pv(j >= 2, s_prev);
       const uint32_t sn = (s + 1 == STAGES) ? 0u : s + 1, phn = (sn == 0) ? ph ^ 1u : ph;
       named_bar_sync(my_turn, 256);
-      mbar_wait(&k_full[sn], phn);
-      wgmma_fence();
-      issue_qk(sn);
-      mbar_wait(&v_full[s], ph);
-      wgmma_fence();  // ptxas would otherwise insert this fence itself after the wait loop
-      issue_pv(pa, s);
-      named_bar_arrive(their_turn, 256);
-      wgmma_wait<1>();  // S_j has landed; PV_{j-1} may still run
-      wgmma_fence_regs(sc);
-      softmax(j);
+      if (Cfg::PV_UNDER_SOFTMAX) {
+        mbar_wait(&k_full[sn], phn);
+        wgmma_fence();
+        issue_qk(sn);
+        mbar_wait(&v_full[s], ph);
+        wgmma_fence();  // ptxas would otherwise insert this fence itself after the wait loop
+        issue_pv(pa, s);
+        named_bar_arrive(next_turn, 256);
+        wgmma_wait<1>();  // S_j has landed; PV_{j-1} may still run
+        wgmma_fence_regs(sc);
+        softmax(j);
+      } else {
+        // PV_{j-1} retires before S_j is issued: P_{j-1} and S_j never hold registers at the same time
+        mbar_wait(&v_full[s], ph);
+        wgmma_fence();
+        issue_pv(pa, s);
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
+        if (lane == 0) mbar_arrive(&kv_empty[s]);
+        mbar_wait(&k_full[sn], phn);
+        wgmma_fence();
+        issue_qk(sn);
+        named_bar_arrive(next_turn, 256);
+        wgmma_wait<0>();
+        wgmma_fence_regs(sc);
+        softmax(j);
+        rescale_pack();
+      }
       s_prev = s;
       s = sn;
       ph = phn;
     }
-    retire_pv(T >= 2, s_prev);
-    // the last PV product; warpgroup 1's turn is the last of all, so it grants none
+    if (Cfg::PV_UNDER_SOFTMAX) retire_pv(T >= 2, s_prev);
+    // the last PV product; the last warpgroup's turn is the last of all, so it grants none
     named_bar_sync(my_turn, 256);
     mbar_wait(&v_full[s], ph);
     wgmma_fence();
     issue_pv(pa, s);
-    if (cw == 0) named_bar_arrive(their_turn, 256);
+    if (cw != NCW - 1) named_bar_arrive(next_turn, 256);
     wgmma_wait<0>();
     wgmma_fence_regs(o);
     if (lane == 0) mbar_arrive(&kv_empty[s]);
@@ -347,7 +403,7 @@ template <int D, bool MASKED>
 static int launch_attention(const idiff_attn_args* a, cudaStream_t stream) {
   using Cfg = AttnCfg<D>;
   CUtensorMap tmQ, tmK0, tmV0, tmK1, tmV1;
-  if (make_head_tmap(&tmQ, a->q, D, a->heads, a->nq, a->batch, a->q_ld, BQ)) return -1;
+  if (make_head_tmap(&tmQ, a->q, D, a->heads, a->nq, a->batch, a->q_ld, Cfg::BQ)) return -1;
   if (make_head_tmap(&tmK0, a->k0, D, a->heads, a->n0, a->batch, a->k0_ld, Cfg::BKV)) return -1;
   if (make_head_tmap(&tmV0, a->v0, D, a->heads, a->n0, a->batch, a->v0_ld, Cfg::BKV)) return -1;
   if (a->n1 > 0) {
@@ -375,8 +431,8 @@ static int launch_attention(const idiff_attn_args* a, cudaStream_t stream) {
                                           Cfg::SMEM_BYTES));
     attr_set = true;
   }
-  dim3 grid((a->nq + BQ - 1) / BQ, a->heads, a->batch);
-  IDIFF_CHECK_CUDA(launch_pdl(attention_kernel<D, MASKED>, dim3(grid), dim3(ATT_THREADS), Cfg::SMEM_BYTES, stream, tmQ,
+  dim3 grid((a->nq + Cfg::BQ - 1) / Cfg::BQ, a->heads, a->batch);
+  IDIFF_CHECK_CUDA(launch_pdl(attention_kernel<D, MASKED>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, tmQ,
                               tmK0, tmV0, tmK1, tmV1, p));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
