@@ -59,6 +59,11 @@ IDIFF_DEVICE void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
                "r"(bytes)
                : "memory");
 }
+// expect `bytes` more transaction bytes in the current phase without arriving (the arrival comes separately)
+IDIFF_DEVICE void mbar_expect_tx_only(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(bytes)
+               : "memory");
+}
 IDIFF_DEVICE void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
 }
@@ -206,6 +211,13 @@ IDIFF_DEVICE float h2f(h16 x) { return __half2float(x); }
 IDIFF_DEVICE h16 f2h(float x) { return __float2half_rn(x); }
 #endif
 IDIFF_DEVICE float silu_f(float x) { return x / (1.0f + __expf(-x)); }
+// LayerNorm scale of a row from its (sum, sum of squares) over K elements: y = rstd * x + nmean
+IDIFF_DEVICE void ln_scale(float sum, float sumsq, int K, float eps, float& rstd, float& nmean) {
+  const float inv_k = 1.0f / (float)K;
+  const float mean = sum * inv_k;
+  rstd = rsqrtf(fmaxf(sumsq * inv_k - mean * mean, 0.f) + eps);
+  nmean = -mean * rstd;
+}
 // Exact (erf) GELU of attention.py:43, x * 0.5 * (1 + erf(x / sqrt 2)), with erf from
 // Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7, far below the fp16 output resolution): one MUFU.RCP,
 // one MUFU.EX2 and ten FMAs instead of libdevice erff (~2x the instructions).  1 + erf is formed

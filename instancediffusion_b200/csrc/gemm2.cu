@@ -25,6 +25,10 @@
 //     mainloop; the store warp writes the buffer out with TMA stores (rows past M / past the conv
 //     image, columns past N clipped by the tensor map) and reloads it for the next tile once the
 //     stores have read it.  Only the final conv's fp32 NCHW output is stored from the fragments.
+//   * compile-time epilogue variants (EPI_*): the feature sets the UNet launches each get a kernel with only
+//     their code, and the store warp puts the tile's bias / LayerNorm-fold / gate / time-embedding vectors in
+//     shared memory during the mainloop, so the consumers' epilogue issues no global load.  Everything else
+//     (SiLU / GELU, NCHW, rare combinations) runs the generic epilogue, which decides at run time.
 // conv3x3 gathers the A tile tap by tap with a 4-D TMA box over the NHWC activation; out-of-image taps
 // are zero-filled by the TMA unit (no im2col buffer, no halo copy).
 #include "../../include/idiff_b200.h"
@@ -77,22 +81,57 @@ constexpr int MODE_GATED = 3;  // bias, gate * gate_b[batch entry] * x + residua
 constexpr int EPI_SLAB_COLS = 32;                        // columns of one epilogue slab / TMA box (64 B rows)
 constexpr int EPI_SLAB_BYTES = BM * EPI_SLAB_COLS * 2;   // 8 KB
 
-template <int BN, int MODE>
+// Epilogue variant (template parameter EPI): the features a launch uses, fixed at compile time so that each
+// kernel carries only their code, and the per-tile vectors they read come from shared memory, loaded by the
+// store warp while the consumers run the mainloop.  EPI_GENERIC instead decides every feature at run time from
+// Params and reads the vectors from global memory: SiLU / GELU, the fp32 NCHW output, batch-invariant statistics
+// and combinations no hot-path layer launches.
+constexpr int EPI_BIAS = 1;      // + bias (GEGLU: value and gate bias)
+constexpr int EPI_LNI = 2;       // LayerNorm fold of the A rows (ln_in / ln_s); never with a residual
+constexpr int EPI_LNO = 4;       // LayerNorm statistics of the output rows (ln_out)
+constexpr int EPI_ROWADD = 8;    // conv3x3 + a row per image (the time embedding); the tile spans <= RA_IMAGES images
+constexpr int EPI_RES = 16;      // gate * x + residual (MODE_GATED: gate * gate_b[batch entry])
+constexpr int EPI_GENERIC = 32;
+constexpr int RA_IMAGES = 2;
+
+// Per-tile vectors of a specialised epilogue in shared memory: fp32 column vectors over the BN accumulator
+// columns (zero past N), each tile row's residual gate (MODE_GATED), and the rowadd rows of the tile's images
+// (16-bit, as stored).  The LayerNorm fold's per-row (rstd, -mean * rstd) rides in the epilogue buffer instead
+// (EPI_LNI excludes a residual): at column chunk 0 of the row, which only the row's own warp overwrites.
+template <int BN, int MODE, int EPI>
+struct Prm {
+  static constexpr bool SPEC = !(EPI & EPI_GENERIC);
+  static constexpr int BIAS = 0;                                                     // float offsets
+  static constexpr int CS = BIAS + (SPEC && (EPI & EPI_BIAS) ? BN : 0);
+  static constexpr int GATE = CS + (SPEC && (EPI & EPI_LNI) ? BN : 0);
+  static constexpr int RA = GATE + (SPEC && MODE == MODE_GATED ? BM : 0);
+  static constexpr int BYTES = RA * 4 + (SPEC && (EPI & EPI_ROWADD) ? RA_IMAGES * BN * 2 : 0);
+};
+
+template <int BN, int MODE, int EPI = EPI_GENERIC>
 struct Cfg {
   static constexpr int B_STAGE_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   // epilogue buffer: the 128 x EW output tile (GEGLU: BN/2 columns; none for the fp32 NCHW output)
   static constexpr int EW = MODE == MODE_NCHW ? 0 : MODE == MODE_GEGLU ? BN / 2 : BN;
   static constexpr int EPI_BYTES = BM * EW * 2;
-  static constexpr int BAR_BYTES = 256;          // 2 * STAGES + 2 mbarriers
-  static constexpr int FIXED = 1024 + BAR_BYTES;  // + slack to align the ring to 1024 B (SWIZZLE_128B)
+  static constexpr int BAR_BYTES = 128;  // 2 * STAGES + 2 mbarriers
+  // + slack to align the ring to 1024 B (SWIZZLE_128B) from the 128 B alignment of the dynamic shared memory
+  // (smem_raw); the GEGLU + LayerNorm-fold variant needs all of it: 4 stages, the 32 KB buffer and 2 KB of
+  // vectors fill the 227 KB exactly
+  static constexpr int FIXED = 1024 - 128 + BAR_BYTES;
+  // the operand ring is sized without the per-tile vectors: they never cost a stage
   static constexpr int STAGES_FIT = (227 * 1024 - FIXED - EPI_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT > 6 ? 6 : STAGES_FIT;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + FIXED;
+  static constexpr int PRM_BYTES = Prm<BN, MODE, EPI>::BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + FIXED + PRM_BYTES;
   static constexpr int ACC = BN / 2;  // fp32 accumulator registers per consumer thread (64 x BN per warpgroup)
   static_assert(STAGES >= 3, "operand ring too shallow");
   static_assert(EW % EPI_SLAB_COLS == 0, "epilogue slabs must tile the output columns exactly");
   static_assert(STAGE_BYTES % 1024 == 0, "the epilogue buffer after the ring must stay 1024 B aligned");
+  static_assert((2 * STAGES + 2) * 8 <= BAR_BYTES, "mbarriers overflow their block");
+  static_assert(SMEM_BYTES <= 227 * 1024, "the per-tile vectors do not fit beside the operand ring");
+  static_assert(!(EPI & EPI_LNI) || (EPI & EPI_GENERIC) || !(EPI & EPI_RES), "LayerNorm fold rows live in the epilogue buffer");
 };
 
 struct Seg {
@@ -150,14 +189,21 @@ IDIFF_DEVICE uint32_t epi_offset(int row, int jj) {
   return (uint32_t)((jj >> 2) * EPI_SLAB_BYTES + row * 64 + (((jj & 3) ^ ((row >> 1) & 3)) << 4));
 }
 
+// EPI: epilogue variant (EPI_* above).
 // LNR: producer LayerNorm statistics of the stored 16-bit values instead of the fp32 results (batch-invariant mode)
-template <int BN, int MODE, bool LNR = false>
+template <int BN, int MODE, int EPI, bool LNR = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
              const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR, const Params p) {
-  using C = Cfg<BN, MODE>;
+  using C = Cfg<BN, MODE, EPI>;
+  using P = Prm<BN, MODE, EPI>;
   constexpr int STAGES = C::STAGES;
-  extern __shared__ uint8_t smem_raw[];
+  constexpr bool GEN = (EPI & EPI_GENERIC) != 0;
+  constexpr bool geglu = (MODE == MODE_GEGLU);
+  constexpr bool nchw = (MODE == MODE_NCHW);
+  constexpr bool gated = (MODE == MODE_GATED);
+  static_assert(GEN || !nchw, "the fp32 NCHW output has no staged epilogue: generic only");
+  extern __shared__ __align__(128) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* sA = smem;
@@ -165,8 +211,10 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   uint8_t* sE = smem + STAGES * C::STAGE_BYTES;  // epilogue buffer (C::EPI_BYTES)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(sE + C::EPI_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* epi_ready = empty_bar + STAGES;  // the tile's residual has landed in sE (or: sE is free, no residual)
-  uint64_t* epi_full = epi_ready + 1;        // the consumers have staged the tile's output in sE
+  // the tile's residual has landed in sE (or: sE is free, no residual) and its per-tile vectors are in sP
+  uint64_t* epi_ready = empty_bar + STAGES;
+  uint64_t* epi_full = epi_ready + 1;  // the consumers have staged the tile's output in sE (and are done with sP)
+  float* sP = reinterpret_cast<float*>(sE + C::EPI_BYTES + C::BAR_BYTES);  // per-tile vectors (P::BYTES)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -224,10 +272,32 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       w0 = tw * p.PW;
     }
   };
+  // output row of tile row rl: its index (rows of the NHWC image for conv3x3), whether it exists, its batch entry
+  // (conv: image) and its position in the entry
+  auto row_of = [&](int rl, int m0, int b0, int h0, int w0, long& orow, bool& rok, int& bidx, int& pix) {
+    if (p.conv) {
+      const int pw = rl % p.PW;
+      const int ph_ = (rl / p.PW) % p.PH;
+      const int pb = rl / (p.PW * p.PH);
+      const int b = b0 + pb, h = h0 + ph_, w = w0 + pw;
+      rok = (b < p.Bn) && (h < p.H) && (w < p.W);
+      pix = h * p.W + w;
+      orow = (long)b * p.H * p.W + pix;
+      bidx = b;
+    } else {
+      orow = (long)m0 + rl;
+      rok = orow < p.M;
+      bidx = (int)(orow / p.rows_per_batch);
+      pix = (int)(orow - (long)bidx * p.rows_per_batch);
+    }
+  };
 
-  // Register split (setmaxnreg at the head of each role branch): 40 x 128 + 232 x 256 <= the CTA's 65536.
+  // Register split (setmaxnreg at the head of each role branch): 96 x 128 + 200 x 256 <= 168 x 384, the registers
+  // the CTA holds from launch (__launch_bounds__(384, 1)); an increase past that pool would never be granted.  ptxas
+  // compiles each role within its share: 96 lets the store warp fill the per-tile vectors without spilling.
+  static_assert(96 * 128 + 200 * 256 <= 168 * THREADS, "register split exceeds the CTA's pool");
   if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 96;\n");
     // ===================== TMA producer =====================
     if (threadIdx.x == 0) {
       WorkIter it(p, cta);
@@ -266,45 +336,93 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           }
         }
       }
-    } else if (C::EW > 0 && warp == 1 && lane == 0) {
-      // ===================== epilogue store warp: residual in, result out =====================
-      // Per owner segment (the ones that run an epilogue): fill sE with the tile's residual (or just
-      // release it to the consumers), wait until they have staged the result there, store it, and wait
-      // until the stores have read sE before the next tile's residual may overwrite it.
+    } else if (C::EW > 0 && warp == 1) {
+      // ===================== epilogue store warp: residual and per-tile vectors in, result out =====================
+      // Per owner segment (the ones that run an epilogue): fill sE with the tile's residual (lane 0, TMA) and sP
+      // with its per-tile vectors (all lanes), release both to the consumers, wait until they have staged the
+      // result in sE (and so are done with sP), store it, and wait until the stores have read sE before the
+      // next tile's residual may overwrite it.  All of it overlaps the consumers' next mainloop.
       WorkIter it(p, cta);
       Seg sg;
       uint32_t ep = 0;
-      const int n_out = MODE == MODE_GEGLU ? p.N / 2 : p.N;
+      const int n_out = geglu ? p.N / 2 : p.N;
       while (it.next(sg)) {
         if (sg.kb0 != 0) continue;
         int n0, m0, b0, h0, w0;
         tile_origin(sg.tile, n0, m0, b0, h0, w0);
-        const int oc0 = MODE == MODE_GEGLU ? (sg.tile % p.n_tiles) * (BN / 2) : n0;
+        const int oc0 = geglu ? (sg.tile % p.n_tiles) * (BN / 2) : n0;
         const int rem = (n_out - oc0 + EPI_SLAB_COLS - 1) / EPI_SLAB_COLS;  // slabs not wholly past N
         const int slabs = rem < C::EW / EPI_SLAB_COLS ? rem : C::EW / EPI_SLAB_COLS;
-        if (p.residual) {
-          mbar_expect_tx(epi_ready, slabs * EPI_SLAB_BYTES);  // clipped box elements count (zero-filled)
+        if (lane == 0 && (GEN ? p.residual != nullptr : (EPI & EPI_RES) != 0)) {
+          mbar_expect_tx_only(epi_ready, slabs * EPI_SLAB_BYTES);  // clipped box elements count (zero-filled)
           for (int q = 0; q < slabs; ++q) {
             if (p.conv) tma_load_4d(sE + q * EPI_SLAB_BYTES, &tmR, epi_ready, oc0 + q * EPI_SLAB_COLS, w0, h0, b0);
             else tma_load_2d(sE + q * EPI_SLAB_BYTES, &tmR, epi_ready, oc0 + q * EPI_SLAB_COLS, m0);
           }
-        } else {
+        }
+        if constexpr (!GEN) {
+          // column vectors over the BN accumulator columns (GEGLU: [value | gate]), zero past N
+          if constexpr ((EPI & (EPI_BIAS | EPI_LNI)) != 0) {
+            for (int c = lane; c < BN; c += 32) {
+              const bool cok = oc0 + (geglu ? c % (BN / 2) : c) < n_out;
+              if constexpr ((EPI & EPI_BIAS) != 0) sP[P::BIAS + c] = cok ? __ldg(p.bias + n0 + c) : 0.f;
+              if constexpr ((EPI & EPI_LNI) != 0) sP[P::CS + c] = cok ? __ldg(p.ln_s + n0 + c) : 0.f;
+            }
+          }
+          if constexpr (gated || (EPI & EPI_LNI) != 0) {
+            for (int rl = lane; rl < BM; rl += 32) {
+              long orow;
+              bool rok;
+              int bidx, pix;
+              row_of(rl, m0, b0, h0, w0, orow, rok, bidx, pix);
+              if constexpr (gated) sP[P::GATE + rl] = rok ? p.gate * __ldg(p.gate_b + bidx) : p.gate;
+              if constexpr ((EPI & EPI_LNI) != 0) {
+                // the row's statistics from the producer GEMM's partial sums, added in slot order (deterministic)
+                float a = 0.f, q = 0.f;
+                if (rok) {
+                  for (int sl = 0; sl < p.ln_slots; ++sl) {
+                    const float2 v = __ldcg(p.ln_in + (long)sl * p.M + orow);
+                    a += v.x;
+                    q += v.y;
+                  }
+                }
+                float2 s;
+                ln_scale(a, q, p.K, p.ln_eps, s.x, s.y);
+                *reinterpret_cast<float2*>(sE + epi_offset(rl, 0)) = s;
+              }
+            }
+          }
+          if constexpr ((EPI & EPI_ROWADD) != 0) {
+            // the rowadd rows of the tile's images, as 16-bit pairs
+            uint32_t* ra = reinterpret_cast<uint32_t*>(sP + P::RA);
+            for (int i = lane; i < RA_IMAGES * BN / 2; i += 32) {
+              const int pb = i / (BN / 2), c = 2 * (i % (BN / 2));
+              const int b = b0 + pb;
+              ra[i] = (b < p.Bn && n0 + c < p.N)
+                          ? __ldg(reinterpret_cast<const uint32_t*>(p.rowadd + (long)b * p.ldra + n0 + c))
+                          : 0u;
+            }
+          }
+        }
+        __syncwarp();
+        if (lane == 0) {
           mbar_arrive(epi_ready);
+          mbar_wait(epi_full, ep);
+          for (int q = 0; q < slabs; ++q) {
+            if (p.conv) tma_store_4d(&tmO, sE + q * EPI_SLAB_BYTES, oc0 + q * EPI_SLAB_COLS, w0, h0, b0);
+            else tma_store_2d(&tmO, sE + q * EPI_SLAB_BYTES, oc0 + q * EPI_SLAB_COLS, m0);
+          }
+          tma_store_commit();
+          stamp_tile(3);
+          tma_store_wait_read();
         }
-        mbar_wait(epi_full, ep);
         ep ^= 1;
-        for (int q = 0; q < slabs; ++q) {
-          if (p.conv) tma_store_4d(&tmO, sE + q * EPI_SLAB_BYTES, oc0 + q * EPI_SLAB_COLS, w0, h0, b0);
-          else tma_store_2d(&tmO, sE + q * EPI_SLAB_BYTES, oc0 + q * EPI_SLAB_COLS, m0);
-        }
-        tma_store_commit();
-        stamp_tile(3);
-        tma_store_wait_read();
+        __syncwarp();  // sE and sP are free again
       }
-      tma_store_wait_all();
+      if (lane == 0) tma_store_wait_all();
     }
   } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 200;\n");
     // ===================== consumers: mainloop + epilogue =====================
     const int cw = (warp >> 2) - 1;  // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
     const int ew = warp - 4;         // consumer warp 0..7
@@ -312,13 +430,10 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     const int t4 = lane & 3;
     // tile rows of this thread (accumulator fragment: wgmma.cuh): rl0 and rl0 + 8
     const int rl0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);
-    constexpr bool geglu = (MODE == MODE_GEGLU);
-    constexpr bool nchw = (MODE == MODE_NCHW);
-    constexpr bool gated = (MODE == MODE_GATED);
     constexpr int NJ = BN / 8;                     // 8-column groups of the accumulator
     constexpr int NJO = geglu ? NJ / 2 : NJ;       // ... that produce output columns
-    const bool do_silu = !gated && (p.flags & IDIFF_EPI_SILU) != 0;
-    const bool do_gelu = !gated && (p.flags & IDIFF_EPI_GELU) != 0;
+    const bool do_silu = GEN && !gated && (p.flags & IDIFF_EPI_SILU) != 0;
+    const bool do_gelu = GEN && !gated && (p.flags & IDIFF_EPI_GELU) != 0;
     const int n_out_total = geglu ? p.N / 2 : p.N;
     // K-major SWIZZLE_128B descriptors of stage 0; a stage / 16-deep k-step is an address offset (>> 4)
     const uint64_t da0 = make_wgmma_desc(smem_u32(sA) + cw * 64 * 128, 16, 1024);
@@ -406,29 +521,13 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       bool rok[2];
       int bidx[2], pix[2];
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int rl = rl0 + 8 * hh;
-        if (p.conv) {
-          const int pw = rl % p.PW;
-          const int ph_ = (rl / p.PW) % p.PH;
-          const int pb = rl / (p.PW * p.PH);
-          const int b = b0 + pb, h = h0 + ph_, w = w0 + pw;
-          rok[hh] = (b < p.Bn) && (h < p.H) && (w < p.W);
-          pix[hh] = h * p.W + w;
-          orow[hh] = (long)b * p.H * p.W + pix[hh];
-          bidx[hh] = b;
-        } else {
-          orow[hh] = (long)m0 + rl;
-          rok[hh] = orow[hh] < p.M;
-          bidx[hh] = (int)(orow[hh] / p.rows_per_batch);
-          pix[hh] = (int)(orow[hh] - (long)bidx[hh] * p.rows_per_batch);
-        }
-      }
+      for (int hh = 0; hh < 2; ++hh) row_of(rl0 + 8 * hh, m0, b0, h0, w0, orow[hh], rok[hh], bidx[hh], pix[hh]);
       // LayerNorm fold, consumer side: each row's mean / rstd from the producer GEMM's partial sums, added in
       // slot order (deterministic).  y = rstd * (x . W'^T - mean * colsum(W')) + (W beta + b).
-      const bool lni = !gated && p.ln_in != nullptr;
+      // (Specialised epilogues read them from sE once the store warp has put them there.)
+      const bool lni = GEN ? !gated && p.ln_in != nullptr : (EPI & EPI_LNI) != 0;
       float ln_rstd[2] = {1.f, 1.f}, ln_nmean[2] = {0.f, 0.f};
-      if (lni) {
+      if (GEN && lni) {
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           float a = 0.f, q = 0.f;
@@ -439,20 +538,18 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
               q += v.y;
             }
           }
-          const float inv_k = 1.0f / (float)p.K;
-          const float mean = a * inv_k;
-          ln_rstd[hh] = rsqrtf(fmaxf(q * inv_k - mean * mean, 0.f) + p.ln_eps);
-          ln_nmean[hh] = -mean * ln_rstd[hh];
+          ln_scale(a, q, p.K, p.ln_eps, ln_rstd[hh], ln_nmean[hh]);
         }
       }
       const int out_col_base = geglu ? (sg.tile % p.n_tiles) * (BN / 2) : n0;
-      const bool has_res = p.residual != nullptr;
-      const bool lno = p.ln_out != nullptr;
+      const bool has_res = GEN ? p.residual != nullptr : (EPI & EPI_RES) != 0;
+      const bool lno = GEN ? p.ln_out != nullptr : (EPI & EPI_LNO) != 0;
+      const bool rowadd = GEN ? !gated && p.rowadd != nullptr : (EPI & EPI_ROWADD) != 0;
       float ln_ps[2] = {0.f, 0.f}, ln_pq[2] = {0.f, 0.f};
       const float gate = p.gate;
       // MODE_GATED: the residual gate of each row is gate * gate_b[its batch entry]
       float gate_r[2] = {gate, gate};
-      if (gated) {
+      if (GEN && gated) {
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh)
           if (rok[hh]) gate_r[hh] = gate * __ldg(p.gate_b + bidx[hh]);
@@ -460,8 +557,19 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       // column vectors of the 8-column group j at this thread's column pair (zero for columns past N)
       auto col_vecs = [&](int j, float2& bv, float2& bg, float2& sv, float2& sgt) {
         const int c = 8 * j + 2 * t4;  // tile column of the pair (GEGLU: value column; its gate is BN/2 further on)
-        const int oc = out_col_base + c;
         bv = bg = sv = sgt = make_float2(0.f, 0.f);
+        if constexpr (!GEN) {
+          if constexpr ((EPI & EPI_BIAS) != 0) {
+            bv = *reinterpret_cast<const float2*>(sP + P::BIAS + c);
+            if (geglu) bg = *reinterpret_cast<const float2*>(sP + P::BIAS + BN / 2 + c);
+          }
+          if constexpr ((EPI & EPI_LNI) != 0) {
+            sv = *reinterpret_cast<const float2*>(sP + P::CS + c);
+            if (geglu) sgt = *reinterpret_cast<const float2*>(sP + P::CS + BN / 2 + c);
+          }
+          return;
+        }
+        const int oc = out_col_base + c;
         if (oc >= n_out_total) return;  // 16-bit outputs have N % 8 == 0: a pair is wholly inside or outside
         const bool hi = !nchw || oc + 1 < n_out_total;  // fp32 NCHW output may have an odd N (the final conv: 3 or 4)
         if (p.bias) {
@@ -498,8 +606,10 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           x0 *= gelu_erf_f(g0);
           x1 *= gelu_erf_f(g1);
         } else {
-          if (!gated && p.rowadd && rok[hh] && out_col_base + 8 * j < n_out_total) {
-            const float2 f = ld_pair(p.rowadd + (long)bidx[hh] * p.ldra + n0 + 8 * j + 2 * t4);
+          if (rowadd && rok[hh] && out_col_base + 8 * j < n_out_total) {
+            const float2 f =
+                GEN ? ld_pair(p.rowadd + (long)bidx[hh] * p.ldra + n0 + 8 * j + 2 * t4)
+                    : unpack_half2(reinterpret_cast<const uint32_t*>(sP + P::RA)[((bidx[hh] - b0) * BN + 8 * j + 2 * t4) / 2]);
             x0 += f.x;
             x1 += f.y;
           }
@@ -540,6 +650,18 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         const uint32_t se = smem_u32(sE);
         mbar_wait(epi_ready, ep);
         ep ^= 1;
+        if constexpr (!GEN && (gated || (EPI & EPI_LNI) != 0)) {
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            if constexpr (gated) gate_r[hh] = sP[P::GATE + rl0 + 8 * hh];
+            if constexpr ((EPI & EPI_LNI) != 0) {
+              const float2 s = *reinterpret_cast<const float2*>(sE + epi_offset(rl0 + 8 * hh, 0));
+              ln_rstd[hh] = s.x;
+              ln_nmean[hh] = s.y;
+            }
+          }
+          __syncwarp();  // the warp's stmatrix below overwrites the rows' statistics
+        }
 #pragma unroll
         for (int jp = 0; jp < NJO / 2; ++jp) {
           const uint32_t addr = se + epi_offset(lrow, 2 * jp + (lane >> 4));
@@ -642,9 +764,9 @@ static int encode_epi_map(CUtensorMap* m, const void* base, int n, int ld, const
   return encode_tmap_f16_sw(m, base, 2, dims, strides, box, 64);
 }
 
-template <int BN, int MODE, bool LNR = false>
+template <int BN, int MODE, int EPI, bool LNR = false>
 static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
-  using C = Cfg<BN, MODE>;
+  using C = Cfg<BN, MODE, EPI>;
   Params p;
   memset(&p, 0, sizeof(p));
   p.M = a->M;
@@ -744,11 +866,11 @@ static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
 
   static bool attr_set = false;
   if (!attr_set) {
-    IDIFF_CHECK_CUDA(cudaFuncSetAttribute(gemm2_kernel<BN, MODE, LNR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    IDIFF_CHECK_CUDA(cudaFuncSetAttribute(gemm2_kernel<BN, MODE, EPI, LNR>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                           C::SMEM_BYTES));
     attr_set = true;
   }
-  IDIFF_CHECK_CUDA(launch_pdl(gemm2_kernel<BN, MODE, LNR>, dim3(p.G), dim3(THREADS), C::SMEM_BYTES, stream, tmA, tmB, tmO, tmR, p));
+  IDIFF_CHECK_CUDA(launch_pdl(gemm2_kernel<BN, MODE, EPI, LNR>, dim3(p.G), dim3(THREADS), C::SMEM_BYTES, stream, tmA, tmB, tmO, tmR, p));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -865,34 +987,88 @@ static Resolved resolve(const idiff_gemm_args* a, bool stats) {
   return {pl.bn, MODE_PLAIN, pl.sk};
 }
 
-template <int MODE>
-static int launch_bn(const idiff_gemm_args* a, cudaStream_t stream, const Resolved& r) {
-  // batch-invariant producers of LayerNorm statistics (resolve caps them at 192)
-  if (batch_invariant() && a->ln_stats_out) {
-    switch (r.bn) {
-      case 192: return launch<192, MODE, true>(a, stream, r.sk);
-      case 160: return launch<160, MODE, true>(a, stream, r.sk);
-      case 128: return launch<128, MODE, true>(a, stream, r.sk);
-      default: return set_error("idiff_gemm: no stored-statistics kernel of tile width %d (resolve caps them at 192)", r.bn);
-    }
+// The epilogue variant of a launch: its exact feature set when that is one the UNet's hot path launches (the
+// instantiations below), else EPI_GENERIC.
+static int epi_variant(const idiff_gemm_args* a, int mode) {
+  if (mode == MODE_NCHW || (a->flags & (IDIFF_EPI_SILU | IDIFF_EPI_GELU))) return EPI_GENERIC;
+  int e = (a->bias ? EPI_BIAS : 0) | (a->residual ? EPI_RES : 0) | (a->ln_stats_out ? EPI_LNO : 0) |
+          (a->ln_stats_in ? EPI_LNI : 0);
+  if (a->rowadd) {
+    if (a->conv_h <= 0) return EPI_GENERIC;
+    int pw, ph, pb;
+    choose_patch(a->conv_h, a->conv_w, &pw, &ph, &pb);
+    if (pb > RA_IMAGES) return EPI_GENERIC;
+    e |= EPI_ROWADD;
   }
+  switch (mode) {
+    case MODE_PLAIN:  // kv / emb; skip, emb and up / down convs; qkv / q; attn-out / proj / ff2; ResBlock conv2; conv1
+      if (e == 0 || e == EPI_BIAS || e == (EPI_BIAS | EPI_LNI) || e == (EPI_BIAS | EPI_RES) ||
+          e == (EPI_BIAS | EPI_RES | EPI_LNO) || e == (EPI_BIAS | EPI_ROWADD))
+        return e;
+      break;
+    case MODE_GATED:  // the fusers' projections
+      if (e == (EPI_BIAS | EPI_RES) || e == (EPI_BIAS | EPI_RES | EPI_LNO)) return e;
+      break;
+    case MODE_GEGLU:  // with and without the LayerNorm fold
+      if (e == EPI_BIAS || e == (EPI_BIAS | EPI_LNI)) return e;
+      break;
+  }
+  return EPI_GENERIC;
+}
+
+template <int MODE, int EPI>
+static int launch_bn(const idiff_gemm_args* a, cudaStream_t stream, const Resolved& r) {
   switch (r.bn) {
     case 256:
-      if constexpr (MODE != MODE_GATED) return launch<256, MODE>(a, stream, r.sk);
+      if constexpr (MODE != MODE_GATED) return launch<256, MODE, EPI>(a, stream, r.sk);
       return -1;  // (resolve never plans it)
-    case 192: return launch<192, MODE>(a, stream, r.sk);
-    case 160: return launch<160, MODE>(a, stream, r.sk);
-    default: return launch<128, MODE>(a, stream, r.sk);
+    case 192: return launch<192, MODE, EPI>(a, stream, r.sk);
+    case 160: return launch<160, MODE, EPI>(a, stream, r.sk);
+    default: return launch<128, MODE, EPI>(a, stream, r.sk);
   }
 }
 
-// One instantiation per (tile width, epilogue mode): each kernel carries only its own mode's code.
+template <int MODE>
+static int launch_lnr(const idiff_gemm_args* a, cudaStream_t stream, const Resolved& r) {
+  switch (r.bn) {
+    case 192: return launch<192, MODE, EPI_GENERIC, true>(a, stream, r.sk);
+    case 160: return launch<160, MODE, EPI_GENERIC, true>(a, stream, r.sk);
+    case 128: return launch<128, MODE, EPI_GENERIC, true>(a, stream, r.sk);
+    default: return set_error("idiff_gemm: no stored-statistics kernel of tile width %d (resolve caps them at 192)", r.bn);
+  }
+}
+
+// One instantiation per (tile width, epilogue mode, epilogue variant): each kernel carries only its own code.
 int gemm_v2(const idiff_gemm_args* a, cudaStream_t stream) {
   const Resolved r = resolve(a, a->ln_stats_out != nullptr);
-  if (r.mode == MODE_GEGLU) return launch<256, MODE_GEGLU>(a, stream, r.sk);
-  if (r.mode == MODE_NCHW) return launch<128, MODE_NCHW>(a, stream, r.sk);
-  if (r.mode == MODE_GATED) return launch_bn<MODE_GATED>(a, stream, r);
-  return launch_bn<MODE_PLAIN>(a, stream, r);
+  if (r.mode == MODE_NCHW) return launch<128, MODE_NCHW, EPI_GENERIC>(a, stream, r.sk);
+  // batch-invariant producers of LayerNorm statistics (resolve caps them at 192)
+  if (batch_invariant() && a->ln_stats_out)
+    return r.mode == MODE_GATED ? launch_lnr<MODE_GATED>(a, stream, r) : launch_lnr<MODE_PLAIN>(a, stream, r);
+  const int e = epi_variant(a, r.mode);
+  if (r.mode == MODE_GEGLU) {
+    switch (e) {
+      case EPI_BIAS: return launch<256, MODE_GEGLU, EPI_BIAS>(a, stream, r.sk);
+      case EPI_BIAS | EPI_LNI: return launch<256, MODE_GEGLU, EPI_BIAS | EPI_LNI>(a, stream, r.sk);
+      default: return launch<256, MODE_GEGLU, EPI_GENERIC>(a, stream, r.sk);
+    }
+  }
+  if (r.mode == MODE_GATED) {
+    switch (e) {
+      case EPI_BIAS | EPI_RES: return launch_bn<MODE_GATED, EPI_BIAS | EPI_RES>(a, stream, r);
+      case EPI_BIAS | EPI_RES | EPI_LNO: return launch_bn<MODE_GATED, EPI_BIAS | EPI_RES | EPI_LNO>(a, stream, r);
+      default: return launch_bn<MODE_GATED, EPI_GENERIC>(a, stream, r);
+    }
+  }
+  switch (e) {
+    case 0: return launch_bn<MODE_PLAIN, 0>(a, stream, r);
+    case EPI_BIAS: return launch_bn<MODE_PLAIN, EPI_BIAS>(a, stream, r);
+    case EPI_BIAS | EPI_LNI: return launch_bn<MODE_PLAIN, EPI_BIAS | EPI_LNI>(a, stream, r);
+    case EPI_BIAS | EPI_RES: return launch_bn<MODE_PLAIN, EPI_BIAS | EPI_RES>(a, stream, r);
+    case EPI_BIAS | EPI_RES | EPI_LNO: return launch_bn<MODE_PLAIN, EPI_BIAS | EPI_RES | EPI_LNO>(a, stream, r);
+    case EPI_BIAS | EPI_ROWADD: return launch_bn<MODE_PLAIN, EPI_BIAS | EPI_ROWADD>(a, stream, r);
+    default: return launch_bn<MODE_PLAIN, EPI_GENERIC>(a, stream, r);
+  }
 }
 
 // slots of the LayerNorm partial statistics a producer GEMM with these arguments writes per row

@@ -126,6 +126,45 @@ if which in ("all", "gemm"):
     tot = sum(r["us"] * r["count"] for r in rows)
     fl = sum(r["us"] * r["count"] * r["tflops"] for r in rows)
     print(f"GEMM+conv per forward (count-weighted): {tot / 1e3:.2f} ms, {fl / tot:.1f} TFLOP/s average")
+    # The epilogues the forward actually runs at the short-K levels (the rows above use plain / residual stand-ins
+    # and stay as they are so that old and new numbers compare).  bound: the larger of FLOPs at 989 TFLOP/s and
+    # bytes at 3.35 TB/s (H100 SXM data sheet), so x bound is how far a launch is from either roof.
+    print(f"{'epilogue variant':30s} {'M':>6s} {'N':>6s} {'K':>6s} {'us':>8s} {'TFLOP/s':>8s} {'GB/s':>8s} {'x bound':>8s}")
+    for hw, C in ((4096, 320), (1024, 640)):
+        M = B * hw
+        a = rnd(M, C)
+        res = rnd(M, C)
+        w = rnd(C, C, scale=1 / math.sqrt(C))
+        bias = torch.randn(C, device=dev)
+        _, st = ops.gemm(a, w, bias, residual=res, want_stats=True)
+        ones = torch.ones(B, device=dev)
+        gamma, beta = torch.ones(C, device=dev), torch.zeros(C, device=dev)
+        fq = ops.fold_layernorm(torch.randn(3 * C, C, device=dev) / math.sqrt(C), None, gamma, beta, 1e-5)
+        fg = ops.fold_layernorm(torch.randn(8 * C, C, device=dev) / math.sqrt(C), torch.randn(8 * C, device=dev),
+                                gamma, beta, 1e-5, pack=pack_geglu)
+        o3 = torch.empty((M, 3 * C), dtype=torch.float16, device=dev)
+        o4 = torch.empty((M, 4 * C), dtype=torch.float16, device=dev)
+        o1 = torch.empty((M, C), dtype=torch.float16, device=dev)
+        wc = rnd(C, 9 * C, scale=1 / math.sqrt(9 * C))
+        emb = rnd(B, C)
+        cases = [  # label, fn, N, K, output columns, bytes beyond A, W and the output
+            (f"qkv LN-fold C{C}", lambda: ops.gemm(a, fq.w, fq.bias, ln=(st, fq.colsum, fq.eps), out=o3), 3 * C, C, 3 * C, 0),
+            (f"geglu LN-fold C{C}", lambda: ops.gemm(a, fg.w, fg.bias, geglu=True, ln=(st, fg.colsum, fg.eps), out=o4),
+             8 * C, C, 4 * C, 0),
+            (f"proj + stats C{C}", lambda: ops.gemm(a, w, bias, residual=res, out=o1, want_stats=True), C, C, C, 2 * M * C),
+            (f"gated proj + stats C{C}", lambda: ops.gemm(a, w, bias, residual=res, gate_rows=ones, rows_per_batch=hw,
+                                                          out=o1, want_stats=True), C, C, C, 2 * M * C),
+            (f"conv + rowadd C{C}", lambda: ops.gemm(a, wc, bias, conv=(B, int(hw ** 0.5), int(hw ** 0.5), C), rowadd=emb,
+                                                     out=o1), C, 9 * C, C, 0),
+        ]
+        for label, fn, N, K, nout, extra in cases:
+            t = timed(fn)
+            fl = 2.0 * M * N * K
+            by = 2.0 * (M * min(K, C) + N * K + M * nout) + extra
+            bound = max(fl / 989e12, by / 3.35e12)
+            rows.append(dict(kind="gemm_variant", label=label, count=0, M=M, N=N, K=K, us=t * 1e6, tflops=fl / t / 1e12,
+                             gbs=by / t / 1e9, bound_us=bound * 1e6))
+            print(f"{label:30s} {M:6d} {N:6d} {K:6d} {t * 1e6:8.1f} {fl / t / 1e12:8.1f} {by / t / 1e9:8.0f} {t / bound:8.2f}")
 
 if which in ("all", "attn"):
     print(f"\n{'attention':30s} {'cnt':>3s} {'Nq':>6s} {'Nkv':>6s} {'d':>4s} {'us':>8s} {'TFLOP/s':>8s}")
