@@ -346,8 +346,68 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       Seg sg;
       uint32_t ep = 0;
       const int n_out = geglu ? p.N / 2 : p.N;
-      while (it.next(sg)) {
-        if (sg.kb0 != 0) continue;
+      auto next_owner = [&]() {
+        while (it.next(sg))
+          if (sg.kb0 == 0) return true;
+        return false;
+      };
+      // The column vectors, row gates and LayerNorm row statistics come from global memory into registers one
+      // tile ahead (pf_*): fetched while the consumers still work on the tile before, with the loads of a tile
+      // independent of each other, so their latency is off the path to epi_ready.  At 5 k-blocks per tile
+      // (C = 320) a chain of dependent loads per row and slot took longer than the mainloop it should hide behind.
+      constexpr int NC = BN / 32, NR = BM / 32;
+      float pf_bias[NC], pf_cs[NC], pf_gate[NR];
+      float2 pf_ln[NR];
+      auto prefetch = [&]() {
+        int n0, m0, b0, h0, w0;
+        tile_origin(sg.tile, n0, m0, b0, h0, w0);
+        const int oc0 = geglu ? (sg.tile % p.n_tiles) * (BN / 2) : n0;
+        // column vectors over the BN accumulator columns (GEGLU: [value | gate]), zero past N
+        if constexpr ((EPI & (EPI_BIAS | EPI_LNI)) != 0) {
+#pragma unroll
+          for (int i = 0; i < NC; ++i) {
+            const int c = lane + 32 * i;
+            const bool cok = oc0 + (geglu ? c % (BN / 2) : c) < n_out;
+            if constexpr ((EPI & EPI_BIAS) != 0) pf_bias[i] = cok ? __ldg(p.bias + n0 + c) : 0.f;
+            if constexpr ((EPI & EPI_LNI) != 0) pf_cs[i] = cok ? __ldg(p.ln_s + n0 + c) : 0.f;
+          }
+        }
+        if constexpr (gated || (EPI & EPI_LNI) != 0) {
+          long orow[NR];
+          bool rok[NR];
+#pragma unroll
+          for (int i = 0; i < NR; ++i) {
+            int bidx, pix;
+            row_of(lane + 32 * i, m0, b0, h0, w0, orow[i], rok[i], bidx, pix);
+            if constexpr (gated) pf_gate[i] = rok[i] ? p.gate * __ldg(p.gate_b + bidx) : p.gate;
+          }
+          if constexpr ((EPI & EPI_LNI) != 0) {
+            // each row's statistics from the producer GEMM's partial sums, added in slot order (deterministic);
+            // the rows of a slot are loaded together
+            float a[NR], q[NR];
+#pragma unroll
+            for (int i = 0; i < NR; ++i) a[i] = q[i] = 0.f;
+            for (int sl = 0; sl < p.ln_slots; ++sl) {
+              float2 v[NR];
+#pragma unroll
+              for (int i = 0; i < NR; ++i)
+                v[i] = rok[i] ? __ldcg(p.ln_in + (long)sl * p.M + orow[i]) : make_float2(0.f, 0.f);
+#pragma unroll
+              for (int i = 0; i < NR; ++i) {
+                a[i] += v[i].x;
+                q[i] += v[i].y;
+              }
+            }
+#pragma unroll
+            for (int i = 0; i < NR; ++i) ln_scale(a[i], q[i], p.K, p.ln_eps, pf_ln[i].x, pf_ln[i].y);
+          }
+        }
+      };
+      bool have = next_owner();
+      if constexpr (!GEN) {
+        if (have) prefetch();
+      }
+      while (have) {
         int n0, m0, b0, h0, w0;
         tile_origin(sg.tile, n0, m0, b0, h0, w0);
         const int oc0 = geglu ? (sg.tile % p.n_tiles) * (BN / 2) : n0;
@@ -361,36 +421,16 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           }
         }
         if constexpr (!GEN) {
-          // column vectors over the BN accumulator columns (GEGLU: [value | gate]), zero past N
-          if constexpr ((EPI & (EPI_BIAS | EPI_LNI)) != 0) {
-            for (int c = lane; c < BN; c += 32) {
-              const bool cok = oc0 + (geglu ? c % (BN / 2) : c) < n_out;
-              if constexpr ((EPI & EPI_BIAS) != 0) sP[P::BIAS + c] = cok ? __ldg(p.bias + n0 + c) : 0.f;
-              if constexpr ((EPI & EPI_LNI) != 0) sP[P::CS + c] = cok ? __ldg(p.ln_s + n0 + c) : 0.f;
-            }
+          // the vectors prefetched for this tile
+#pragma unroll
+          for (int i = 0; i < NC; ++i) {
+            if constexpr ((EPI & EPI_BIAS) != 0) sP[P::BIAS + lane + 32 * i] = pf_bias[i];
+            if constexpr ((EPI & EPI_LNI) != 0) sP[P::CS + lane + 32 * i] = pf_cs[i];
           }
-          if constexpr (gated || (EPI & EPI_LNI) != 0) {
-            for (int rl = lane; rl < BM; rl += 32) {
-              long orow;
-              bool rok;
-              int bidx, pix;
-              row_of(rl, m0, b0, h0, w0, orow, rok, bidx, pix);
-              if constexpr (gated) sP[P::GATE + rl] = rok ? p.gate * __ldg(p.gate_b + bidx) : p.gate;
-              if constexpr ((EPI & EPI_LNI) != 0) {
-                // the row's statistics from the producer GEMM's partial sums, added in slot order (deterministic)
-                float a = 0.f, q = 0.f;
-                if (rok) {
-                  for (int sl = 0; sl < p.ln_slots; ++sl) {
-                    const float2 v = __ldcg(p.ln_in + (long)sl * p.M + orow);
-                    a += v.x;
-                    q += v.y;
-                  }
-                }
-                float2 s;
-                ln_scale(a, q, p.K, p.ln_eps, s.x, s.y);
-                *reinterpret_cast<float2*>(sE + epi_offset(rl, 0)) = s;
-              }
-            }
+#pragma unroll
+          for (int i = 0; i < NR; ++i) {
+            if constexpr (gated) sP[P::GATE + lane + 32 * i] = pf_gate[i];
+            if constexpr ((EPI & EPI_LNI) != 0) *reinterpret_cast<float2*>(sE + epi_offset(lane + 32 * i, 0)) = pf_ln[i];
           }
           if constexpr ((EPI & EPI_ROWADD) != 0) {
             // the rowadd rows of the tile's images, as 16-bit pairs
@@ -405,8 +445,12 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           }
         }
         __syncwarp();
+        if (lane == 0) mbar_arrive(epi_ready);
+        have = next_owner();  // (sg moves on; this tile's origin is in the locals above)
+        if constexpr (!GEN) {
+          if (have) prefetch();
+        }
         if (lane == 0) {
-          mbar_arrive(epi_ready);
           mbar_wait(epi_full, ep);
           for (int q = 0; q < slabs; ++q) {
             if (p.conv) tma_store_4d(&tmO, sE + q * EPI_SLAB_BYTES, oc0 + q * EPI_SLAB_COLS, w0, h0, b0);
