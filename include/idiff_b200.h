@@ -221,6 +221,20 @@ int idiff_plms_update(const float* x, const float* e_c, const float* e_u, float 
                       const float* old1, const float* old2, const float* old3, float c0, float c1,
                       float c2, float c3, float a_t, float a_prev, float sqrt_one_minus_at,
                       float* e_out, float* x_out, long n, void* stream);
+/* ---------------------------------------------------------------------------------------------
+ * idiff_ddim_update: fused DDIM step (ddim.py:116-131), all fp32, n elements:
+ *   e      = e_u + gs*(e_c - e_u)         (CFG; e_u may be NULL -> e = e_c)
+ *   pred0  = (x - sqrt(1-a_t)*e) / sqrt(a_t)
+ *   x_out  = sqrt(a_prev)*pred0 + sqrt(max(1-a_prev-sigma^2, 0))*e + sigma*z_i
+ * z_i (drawn only for sigma > 0) is a standard normal that depends on (seed, index, i) alone: Philox4x32-10 with key
+ * (seed & 0xffffffff, seed >> 32) and counter (c & 0xffffffff, c >> 32, index, 0), c = i/4, whose four words v0..v3
+ * give elements 4c..4c+3 by Box-Muller on (v0, v1) and (v2, v3): u = (v + 0.5)*2^-32, r = sqrt(-2 ln u_a),
+ * z = r cos(2 pi u_b), then r sin(2 pi u_b).  With x = 0, e_c = 0, e_u = NULL and sigma = 1, x_out is z.
+ * e_out (may be NULL) receives the post-CFG e.
+ * ------------------------------------------------------------------------------------------- */
+int idiff_ddim_update(const float* x, const float* e_c, const float* e_u, float gs, float a_t, float a_prev,
+                      float sigma, unsigned long long seed, int index, float* e_out, float* x_out, long n,
+                      void* stream);
 /* out = mean over `count` latents given as an array of device pointers (plms_instance.py:135) */
 int idiff_latent_mean(const float* const* xs_dev, int count, float* out, long n, void* stream);
 

@@ -78,6 +78,7 @@ SIGNATURES = {
     "idiff_im2col_s2_pad01": (_i, [_vp, _vp, _i, _i, _i, _i, _vp]),
     "idiff_fourier_embed": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "idiff_plms_update": (_i, [_vp, _vp, _vp, _f, _vp, _vp, _vp, _f, _f, _f, _f, _f, _f, _f, _vp, _vp, _l, _vp]),
+    "idiff_ddim_update": (_i, [_vp, _vp, _vp, _f, _f, _f, _f, C.c_uint64, _i, _vp, _vp, _l, _vp]),
     "idiff_latent_mean": (_i, [_vp, _i, _vp, _l, _vp]),
     "idiff_conv_in_select": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "idiff_timestep_embedding": (_i, [_vp, _vp, _i, _i, _vp]),

@@ -243,4 +243,31 @@ IDIFF_DEVICE float exp2_approx(float x) {
   return y;
 }
 
+// Philox4x32-10 (Salmon et al., SC'11; the Random123 constants): a counter-based generator, so a draw is a pure
+// function of (counter, key) and needs no state carried between launches.
+IDIFF_DEVICE uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u;
+    k.y += 0xBB67AE85u;
+  }
+  return c;
+}
+// uint32 -> uniform (v + 0.5) * 2^-32 in (0, 1), rounded to fp32
+IDIFF_DEVICE float u01_open(uint32_t v) { return ((float)v + 0.5f) * 2.3283064365386963e-10f; }
+// Box-Muller on two uniform words: z0 = r cos(2 pi u_b), z1 = r sin(2 pi u_b), r = sqrt(-2 ln u_a), u = (v + 0.5) 2^-32.
+// For u_a above 1/2, ln u_a is log1p(-(1 - u_a)) with 1 - u_a = (~a + 0.5) 2^-32 formed exactly, so small radii keep
+// their precision (u_a rounded to fp32 would lose most of the bits of 1 - u_a).  Precise logf / sincospif throughout.
+IDIFF_DEVICE void box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
+  const float ln_u = a < 0x80000000u ? logf(u01_open(a)) : log1pf(-u01_open(~a));
+  const float r = sqrtf(-2.0f * ln_u);
+  float s, c;
+  sincospif(2.0f * u01_open(b), &s, &c);
+  z0 = r * c;
+  z1 = r * s;
+}
+
 }  // namespace idiff

@@ -182,6 +182,44 @@ __global__ void plms_update_kernel(const float* __restrict__ x, const float* __r
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// fused DDIM update (ddim.py:116-131) with its eta noise drawn in place
+// ---------------------------------------------------------------------------------------------
+// One thread per group of four elements 4c .. 4c+3: Philox4x32-10 at counter (c lo, c hi, index, 0) and key
+// (seed lo, seed hi) gives four words, Box-Muller on (v0, v1) and (v2, v3) their four normals.  So z_i depends on
+// (seed, index, i) only, not on the launch shape, the tensor length beyond i or the batch.  sigma == 0 draws nothing.
+__global__ void ddim_update_kernel(const float* __restrict__ x, const float* __restrict__ e_c,
+                                   const float* __restrict__ e_u, float gs, float sqrt_at, float sqrt_1m_at,
+                                   float sqrt_aprev, float sqrt_dir, float sigma, uint2 key, uint32_t index,
+                                   float* __restrict__ e_out, float* __restrict__ x_out, long n) {
+  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
+  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
+  const long groups = (n + 3) / 4;
+  for (long c = (long)blockIdx.x * blockDim.x + threadIdx.x; c < groups; c += (long)gridDim.x * blockDim.x) {
+    float z[4] = {0.f, 0.f, 0.f, 0.f};
+    if (sigma > 0.f) {
+      const uint4 v = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)((unsigned long long)c >> 32), index, 0u), key);
+      box_muller(v.x, v.y, z[0], z[1]);
+      box_muller(v.z, v.w, z[2], z[3]);
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long i = 4 * c + j;
+      if (i >= n) break;
+      float e = e_c[i];
+      if (e_u) {
+        const float u = e_u[i];
+        e = u + gs * (e - u);
+      }
+      const float pred_x0 = (x[i] - sqrt_1m_at * e) / sqrt_at;
+      float xp = sqrt_aprev * pred_x0 + sqrt_dir * e;
+      if (sigma > 0.f) xp += sigma * z[j];
+      if (e_out) e_out[i] = e;
+      x_out[i] = xp;
+    }
+  }
+}
+
 __global__ void latent_mean_kernel(const float* const* __restrict__ xs, int count, float* __restrict__ out,
                                    long n) {
   pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
@@ -401,6 +439,23 @@ extern "C" int idiff_plms_update(const float* x, const float* e_c, const float* 
                                  float sqrt_one_minus_at, float* e_out, float* x_out, long n, void* stream) {
   IDIFF_REQUIRE(x && e_c && x_out && n > 0, "idiff_plms_update: bad arguments");
   IDIFF_CHECK_CUDA(launch_pdl(plms_update_kernel, dim3(grid_for(n, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  x, e_c, e_u, gs, old1, old2, old3, c0, c1, c2, c3, sqrtf(a_t), sqrtf(a_prev), sqrt_one_minus_at, sqrtf(1.0f - a_prev), e_out, x_out, n));
+  IDIFF_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int idiff_ddim_update(const float* x, const float* e_c, const float* e_u, float gs, float a_t,
+                                 float a_prev, float sigma, unsigned long long seed, int index, float* e_out,
+                                 float* x_out, long n, void* stream) {
+  IDIFF_REQUIRE(x && e_c && x_out && n > 0 && index >= 0 && a_t > 0.f && sigma >= 0.f,
+                "idiff_ddim_update: bad arguments");
+  // the fp32 coefficients of ddim.py:118-129: sqrt(1 - a_prev - sigma^2) clamped at 0 (eta <= 1 keeps it >= 0 up to
+  // rounding)
+  const float sqrt_dir = sqrtf(fmaxf(1.0f - a_prev - sigma * sigma, 0.0f));
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  const long groups = (n + 3) / 4;
+  IDIFF_CHECK_CUDA(launch_pdl(ddim_update_kernel, dim3(grid_for(groups, 256)), dim3(256), 0,
+                              reinterpret_cast<cudaStream_t>(stream), x, e_c, e_u, gs, sqrtf(a_t), sqrtf(1.0f - a_t),
+                              sqrtf(a_prev), sqrt_dir, sigma, key, (uint32_t)index, e_out, x_out, n));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -6,7 +6,7 @@ SURVEY.md section 8b resolve to this package's mirrors:
     ldm.util
     ldm.modules.attention
     ldm.modules.diffusionmodules.{openaimodel, text_grounding_net, util, convnext}
-    ldm.models.diffusion.{plms, plms_instance, ldm, ddpm}
+    ldm.models.diffusion.{plms, plms_instance, ddim, ldm, ddpm}
     grounding_input.text_grounding_tokinzer_input
     utils.model  (set_alpha_scale / alpha_generator only; everything else stays the reference's)
     ldm.models.autoencoder, ldm.modules.diffusionmodules.model   (first stage: AutoencoderKL.decode right
@@ -40,6 +40,7 @@ _MAP = {
     "ldm.modules.diffusionmodules.convnext": "instancediffusion_b200.ldm.modules.diffusionmodules.convnext",
     "ldm.models.diffusion.plms": "instancediffusion_b200.ldm.models.diffusion.plms",
     "ldm.models.diffusion.plms_instance": "instancediffusion_b200.ldm.models.diffusion.plms_instance",
+    "ldm.models.diffusion.ddim": "instancediffusion_b200.ldm.models.diffusion.ddim",
     "ldm.models.diffusion.ldm": "instancediffusion_b200.ldm.models.diffusion.ldm",
     "ldm.models.diffusion.ddpm": "instancediffusion_b200.ldm.models.diffusion.ddpm",
     "grounding_input.text_grounding_tokinzer_input": "instancediffusion_b200.grounding_input.text_grounding_tokinzer_input",

@@ -8,13 +8,14 @@ schedule) and first-conv state.  Per request the arithmetic is that of its own s
 PLMS updates are `PLMSBase._step_predict` / `_step_finish` on its own trajectories with its own guidance scale,
 and a Multi-instance request merges its latents with `ops.latent_mean` at its own step int(steps * mis), where
 steps is the length of the PLMS schedule (`schedule_steps`: S + 1 for some S, e.g. 31 for S = 30), as there.
-That per-request machinery is `_RequestState`, which `SamplingEngine` (engine.py) drives too: `sample_requests` is
-the lock-step driver on top of it.
+A DDIM request (`sampler="ddim"`) takes `DDIMBase`'s one-evaluation update instead, its eta noise keyed by its own seed
+and the step, so it does not depend on the other requests.  That per-request machinery is `_RequestState`, which
+`SamplingEngine` (engine.py) drives too: `sample_requests` is the lock-step driver on top of it.
 
 Contract: each returned latent equals, within floating-point tolerance, what `PLMSSampler.sample()` (input dict,
-mis = 0) or `PLMSSamplerInst.sample()` (input list [global, instance_1 .. instance_n]) returns for that request
-alone on the model in the state it had when `sample_requests` was called.  Afterwards the model's fuser scale and
-first-conv swap are what a sequential run of the same requests would leave.
+mis = 0), `PLMSSamplerInst.sample()` (input list [global, instance_1 .. instance_n]) or `DDIMSampler.sample(eta=,
+seed=)` returns for that request alone on the model in the state it had when `sample_requests` was called.
+Afterwards the model's fuser scale and first-conv swap are what a sequential run of the same requests would leave.
 """
 from __future__ import annotations
 
@@ -29,6 +30,7 @@ from .... import ops
 from ...modules.attention import GatedSelfAttentionDense
 from ...modules.diffusionmodules.util import make_ddim_timesteps
 from ._plms_common import PLMSBase, Trajectory
+from .ddim import DDIMBase, resolve_seed
 
 
 @dataclass
@@ -37,7 +39,9 @@ class Request:
     of `PLMSSamplerInst.sample`; `shape`: (B, 4, H, W) of its latent (may be omitted when input x is given);
     `mis`: the Multi-instance fraction (list inputs only).  `S`: the request's step count; `sample_requests` takes it
     from the call (S, if given, must equal it), `SamplingEngine` requires it.  `mask` / `x0` (inpainting) are not
-    supported and raise."""
+    supported and raise.  `sampler`: "plms", or "ddim" (`DDIMSampler.sample`: input dict only) with its `eta` and
+    `seed` (None at eta > 0: one draw from torch's default CPU generator when `sample_requests` starts or at `submit`,
+    in request order)."""
     input: Union[dict, List[dict]]
     uc: Optional[torch.Tensor] = None
     guidance_scale: float = 1.0
@@ -47,6 +51,12 @@ class Request:
     S: Optional[int] = None
     mask: Optional[torch.Tensor] = None
     x0: Optional[torch.Tensor] = None
+    sampler: str = "plms"
+    eta: float = 0.0
+    seed: Optional[int] = None
+
+
+SAMPLERS = ("plms", "ddim")
 
 
 @dataclass(frozen=True)
@@ -118,6 +128,17 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
         if req.mask is not None or req.x0 is not None:
             raise ValueError(f"request {j}: mask / x0 inpainting is not supported by sample_requests")
         multi = isinstance(req.input, (list, tuple))
+        if req.sampler not in SAMPLERS:
+            raise ValueError(f"request {j}: unknown sampler {req.sampler!r} (have {', '.join(SAMPLERS)})")
+        if not req.eta >= 0:
+            raise ValueError(f"request {j}: eta={req.eta} must be >= 0")
+        if req.sampler == "plms" and req.eta != 0:
+            raise ValueError(f"request {j}: eta={req.eta} needs sampler='ddim' (PLMS is deterministic, eta = 0)")
+        if req.sampler == "ddim" and (multi or req.mis != 0):
+            raise ValueError(f"request {j}: DDIM takes one input dict with mis = 0; the Multi-instance Sampler "
+                             "(input list, mis) is PLMS only")
+        if req.seed is not None and not 0 <= int(req.seed) < 1 << 64:
+            raise ValueError(f"request {j}: seed {req.seed} outside [0, 2^64)")
         if not multi and req.mis != 0:
             raise ValueError(f"request {j}: mis={req.mis} needs the input list [global, inst_1 .. inst_n]; "
                              "a single input dict runs plain PLMS (mis = 0)")
@@ -149,15 +170,21 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
 
 
 class _RequestState:
-    """One request being sampled by `sample_requests` or `SamplingEngine`: its plan and its own PLMS schedule
-    (`make_schedule(S)`), what the model was when the request was admitted, and, once started, its trajectories and its
-    position in the schedule.  Both drivers evaluate a request the same way: `begin`, one forward of its trajectories at
-    `fuser_scale()` and `conv_flag(...)`, `advance` with the eps; after the last step `finish` returns its latent."""
+    """One request being sampled by `sample_requests` or `SamplingEngine`: its plan and its own schedule
+    (`make_schedule(S)` of `PLMSBase`, or of `DDIMBase` with the request's eta and seed), what the model was when the
+    request was admitted, and, once started, its trajectories and its position in the schedule.  Both drivers evaluate a
+    request the same way: `begin`, one forward of its trajectories at `fuser_scale()` and `conv_flag(...)`, `advance`
+    with the eps; after the last step `finish` returns its latent."""
 
     def __init__(self, req: Request, plan: RequestPlan, S: int, model, diffusion):
         self.req, self.plan = req, plan
-        self.base = PLMSBase(diffusion, model)
-        self.base.make_schedule(ddim_num_steps=int(S))
+        if req.sampler == "ddim":
+            self.base = DDIMBase(diffusion, model)
+            self.base.make_schedule(ddim_num_steps=int(S), ddim_eta=float(req.eta))
+            self.base.seed = resolve_seed(self.base.ddim_eta, req.seed)
+        else:
+            self.base = PLMSBase(diffusion, model)
+            self.base.make_schedule(ddim_num_steps=int(S))
         self.time_range = np.flip(self.base.ddim_timesteps)
         self.steps = len(self.time_range)
         self.alphas = req.alpha_generator_func(self.steps) if req.alpha_generator_func is not None else None
@@ -322,8 +349,8 @@ class _RequestState:
 @torch.no_grad()
 def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], S: int, *,
                     max_batch: int = 32) -> List[torch.Tensor]:
-    """Sample every request in `requests` (Request objects or dicts of its fields) with S PLMS steps; returns one
-    latent per request, in order.  `max_batch` bounds the images of one UNet forward.
+    """Sample every request in `requests` (Request objects or dicts of its fields) with S steps of its sampler; returns
+    one latent per request, in order.  `max_batch` bounds the images of one UNet forward.
 
     The per-image fuser scales are those `utils.model.set_alpha_scale` sets (every gated fuser at the request's
     alpha), and the model is left with that function's result for the last alpha of the last request that has an

@@ -10,10 +10,12 @@ when the slowest one finishes.  `SamplingEngine` lets requests join and leave be
 
 A tick gives every live trajectory exactly one UNet evaluation: the one at t of its current step or, for a request
 in the Euler predictor of its first PLMS step, the corrector's evaluation at t_next (so the corrector rides in the
-next tick with everyone else).  Each request is a `batched._RequestState`, the per-request sampling state that
-`sample_requests` drives too: its own schedule (`PLMSBase.make_schedule(S)`), its sampler's arithmetic
-(`PLMSBase._step_predict` / `_step_finish`) and its Multi-instance merge before step int(schedule_steps(S) * mis),
-after the last one for mis = 1.  The engine adds admission, the grouping of a tick's forwards and retirement.
+next tick with everyone else).  A PLMS request therefore retires after schedule_steps(S) + 1 ticks, a DDIM request
+(one evaluation per step) after schedule_steps(S).  Each request is a `batched._RequestState`, the per-request sampling
+state that `sample_requests` drives too: its own schedule (`make_schedule(S)` of `PLMSBase`, or of `DDIMBase` with its
+eta and seed), its sampler's arithmetic (`_step_predict` / `_step_finish`) and its Multi-instance merge before step
+int(schedule_steps(S) * mis), after the last one for mis = 1.  PLMS and DDIM requests of one latent size and context
+length share forwards.  The engine adds admission, the grouping of a tick's forwards and retirement.
 
 The evaluations of a tick are grouped by (latent H x W, context length) in admission order, split into forwards of
 at most `max_batch` images by `plan_chunks`, and each forward is padded to the smallest of `buckets` that holds it.
@@ -23,8 +25,8 @@ context length, mask presence and fuser state (off / per image / one common scal
 The engine never calls set_alpha_scale or swaps the model's first conv.
 
 Contract: each returned latent equals, within floating-point tolerance, what the request's own
-`PLMSSampler.sample()` / `PLMSSamplerInst.sample()` returns when it runs alone on the model in the state it had at
-`submit`, whatever else is live and whenever the request arrived.
+`PLMSSampler.sample()` / `PLMSSamplerInst.sample()` / `DDIMSampler.sample(eta=, seed=)` returns when it runs alone on
+the model in the state it had at `submit`, whatever else is live and whenever the request arrived.
 """
 from __future__ import annotations
 

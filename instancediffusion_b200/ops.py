@@ -487,6 +487,25 @@ def plms_update(x: torch.Tensor, e_c: torch.Tensor, e_u: Optional[torch.Tensor],
           "idiff_plms_update")
 
 
+def ddim_update(x: torch.Tensor, e_c: torch.Tensor, e_u: Optional[torch.Tensor], gs: float, a_t: float,
+                a_prev: float, sigma: float, seed: int, index: int, e_out: Optional[torch.Tensor],
+                x_out: torch.Tensor) -> None:
+    """One DDIM step (include/idiff_b200.h idiff_ddim_update): fp32 contiguous tensors of one size; the noise of
+    sigma > 0 is a function of (seed, index, element) only.  seed: an integer in [0, 2^64)."""
+    lib = _lib.load()
+    for name, t in (("x", x), ("e_c", e_c), ("e_u", e_u), ("e_out", e_out), ("x_out", x_out)):
+        if t is not None:
+            _req(t, torch.float32, name)
+            if t.numel() != x.numel() or not t.is_contiguous():
+                raise _lib.IdiffError(f"ddim_update: {name} must be contiguous with {x.numel()} elements")
+    seed = int(seed)
+    if not 0 <= seed < 1 << 64:
+        raise _lib.IdiffError(f"ddim_update: seed {seed} outside [0, 2^64)")
+    check(lib.idiff_ddim_update(x.data_ptr(), e_c.data_ptr(), _ptr(e_u), float(gs), float(a_t), float(a_prev),
+                                float(sigma), seed, int(index), _ptr(e_out), x_out.data_ptr(), x.numel(), _stream()),
+          "idiff_ddim_update")
+
+
 def latent_mean(xs, out: torch.Tensor) -> torch.Tensor:
     lib = _lib.load()
     ptrs = torch.tensor([t.data_ptr() for t in xs], dtype=torch.int64).to(out.device)
