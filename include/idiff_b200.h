@@ -235,6 +235,16 @@ int idiff_plms_update(const float* x, const float* e_c, const float* e_u, float 
 int idiff_ddim_update(const float* x, const float* e_c, const float* e_u, float gs, float a_t, float a_prev,
                       float sigma, unsigned long long seed, int index, float* e_out, float* x_out, long n,
                       void* stream);
+/* ---------------------------------------------------------------------------------------------
+ * idiff_noise_latent: start latent of image-to-image sampling (SDEdit), all fp32, n elements:
+ *   x_out[i] = sqrt_a*x_init[i % n_init] + sqrt_1m_a*z_i          (n % n_init == 0: x_init broadcast over the batch)
+ * z_i is a standard normal that depends on (seed, i) alone: Philox4x32-10 with key (seed & 0xffffffff, seed >> 32)
+ * and counter (c & 0xffffffff, c >> 32, 0, 1), c = i/4, then Box-Muller on the four words exactly as in
+ * idiff_ddim_update.  Counter word 3 is 1 here and 0 there, so the two streams never share a counter and one seed can
+ * key both.  With x_init = 0, sqrt_a = 0 and sqrt_1m_a = 1, x_out is z.
+ * ------------------------------------------------------------------------------------------- */
+int idiff_noise_latent(const float* x_init, long n_init, float sqrt_a, float sqrt_1m_a, unsigned long long seed,
+                       float* x_out, long n, void* stream);
 /* out = mean over `count` latents given as an array of device pointers (plms_instance.py:135) */
 int idiff_latent_mean(const float* const* xs_dev, int count, float* out, long n, void* stream);
 

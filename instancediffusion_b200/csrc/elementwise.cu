@@ -220,6 +220,31 @@ __global__ void ddim_update_kernel(const float* __restrict__ x, const float* __r
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// image-to-image start latent: x_init noised to the start timestep (q_sample with a seeded z)
+// ---------------------------------------------------------------------------------------------
+// One thread per group of four elements 4c .. 4c+3: Philox4x32-10 at counter (c lo, c hi, 0, 1) and key (seed lo,
+// seed hi), Box-Muller as in ddim_update_kernel.  Counter word 3 = 1 keeps the stream disjoint from the DDIM eta
+// noise (word 3 = 0), so one seed can key both.  x_init is broadcast over the batch: element i reads i % n_init.
+__global__ void noise_latent_kernel(const float* __restrict__ x_init, long n_init, float sqrt_a, float sqrt_1m_a,
+                                    uint2 key, float* __restrict__ x_out, long n) {
+  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
+  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
+  const long groups = (n + 3) / 4;
+  for (long c = (long)blockIdx.x * blockDim.x + threadIdx.x; c < groups; c += (long)gridDim.x * blockDim.x) {
+    float z[4];
+    const uint4 v = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)((unsigned long long)c >> 32), 0u, 1u), key);
+    box_muller(v.x, v.y, z[0], z[1]);
+    box_muller(v.z, v.w, z[2], z[3]);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long i = 4 * c + j;
+      if (i >= n) break;
+      x_out[i] = sqrt_a * x_init[i % n_init] + sqrt_1m_a * z[j];
+    }
+  }
+}
+
 __global__ void latent_mean_kernel(const float* const* __restrict__ xs, int count, float* __restrict__ out,
                                    long n) {
   pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
@@ -456,6 +481,18 @@ extern "C" int idiff_ddim_update(const float* x, const float* e_c, const float* 
   IDIFF_CHECK_CUDA(launch_pdl(ddim_update_kernel, dim3(grid_for(groups, 256)), dim3(256), 0,
                               reinterpret_cast<cudaStream_t>(stream), x, e_c, e_u, gs, sqrtf(a_t), sqrtf(1.0f - a_t),
                               sqrtf(a_prev), sqrt_dir, sigma, key, (uint32_t)index, e_out, x_out, n));
+  IDIFF_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int idiff_noise_latent(const float* x_init, long n_init, float sqrt_a, float sqrt_1m_a,
+                                  unsigned long long seed, float* x_out, long n, void* stream) {
+  IDIFF_REQUIRE(x_init && x_out && n > 0 && n_init > 0 && n % n_init == 0, "idiff_noise_latent: bad arguments");
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  const long groups = (n + 3) / 4;
+  IDIFF_CHECK_CUDA(launch_pdl(noise_latent_kernel, dim3(grid_for(groups, 256)), dim3(256), 0,
+                              reinterpret_cast<cudaStream_t>(stream), x_init, n_init, sqrt_a, sqrt_1m_a, key, x_out,
+                              n));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

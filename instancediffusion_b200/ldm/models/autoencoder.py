@@ -54,7 +54,8 @@ class AutoencoderKL(PackedModule):
 
     @torch.no_grad()
     def encode(self, x):
-        """autoencoder.py:27-31 (not on the sampling path; provided for completeness of the module)."""
+        """autoencoder.py:27-31.  Not on the sampling path from noise; its latent can start image-to-image sampling
+        (the samplers' and `Request`'s `x_init`)."""
         h = self.encoder(x)
         moments = torch.nn.functional.conv2d(h, self.quant_conv.weight.float(), self.quant_conv.bias.float())
         return DiagonalGaussianDistribution(moments).sample() * self.scale_factor

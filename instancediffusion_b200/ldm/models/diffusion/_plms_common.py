@@ -6,10 +6,13 @@ GPU-first restructuring of `p_sample_plms` (plms.py:117-167 == plms_instance.py:
   * classifier-free guidance, the Adams-Bashforth combination and the x_{t-1} update are one fused
     kernel (idiff_plms_update) instead of ~12 elementwise launches + deepcopy + 4 torch.full;
   * the schedule scalars are host floats taken from the same fp32 buffers the reference reads.
+
+It also holds what every sampler shares for image-to-image sampling (SDEdit, not in the reference): the start step of
+a strength, the noised start latent and the Multi-instance rule for a truncated schedule.
 """
 from __future__ import annotations
 
-from typing import List
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -25,6 +28,19 @@ _AB = {
 }
 
 
+def resolve_seed(noisy: bool, seed: Optional[int]) -> int:
+    """The seed of a run: `seed` if given; for a run that draws noise (DDIM at eta > 0, image-to-image) otherwise one
+    draw from torch's default CPU generator; 0 for a run without noise (the generator is left untouched)."""
+    if seed is not None:
+        seed = int(seed)
+        if not 0 <= seed < 1 << 64:
+            raise ValueError(f"seed {seed} outside [0, 2^64)")
+        return seed
+    if not noisy:
+        return 0
+    return int(torch.randint(0, 2 ** 63 - 1, (1,), dtype=torch.int64).item())
+
+
 class Trajectory:
     """One denoising trajectory: its input dict (mutated like the reference does: `x`,
     `timesteps`) and its history of post-CFG eps (at most 3, plms.py:109-111)."""
@@ -35,6 +51,8 @@ class Trajectory:
 
 
 class PLMSBase(object):
+    seed = 0  # keys the image-to-image start noise (and DDIMBase's eta noise)
+
     def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None):
         super().__init__()
         self.diffusion = diffusion
@@ -167,3 +185,54 @@ class PLMSBase(object):
         ts = torch.full((b,), step, device=self.device, dtype=torch.long)
         ts_next = torch.full((b,), nxt, device=self.device, dtype=torch.long)
         return ts, ts_next
+
+    # ------------------------------------------------------------------------------------------
+    # image-to-image (SDEdit): start from x_init noised to the step where `strength` of the schedule remains
+    # ------------------------------------------------------------------------------------------
+    @staticmethod
+    def start_step(steps: int, strength: float) -> int:
+        """k0 = N - int(N * strength) for a schedule of N steps: the first step an image-to-image run takes."""
+        strength = float(strength)
+        if not 0 < strength <= 1:
+            raise ValueError(f"strength={strength} outside (0, 1]")
+        n_run = int(steps * strength)
+        if n_run < 1:
+            raise ValueError(f"strength={strength} runs int({steps} * {strength}) = 0 of the {steps} steps")
+        return steps - n_run
+
+    @staticmethod
+    def mis_merge_step(steps: int, mis: float, k0: int, img2img: bool) -> Optional[int]:
+        """Step before which the Multi-instance trajectories merge: int(N * mis), or None when an image-to-image run
+        starts at or after it.  All trajectories would start from the same latent there, and their mean is that latent
+        only in exact arithmetic, so only the global trajectory runs."""
+        merge = int(steps * mis)
+        return None if img2img and merge <= k0 else merge
+
+    def check_init(self, shape, x_init, strength) -> int:
+        """Validate the image-to-image arguments of a run of latent `shape` on the current schedule; returns k0
+        (0 without x_init, which needs strength 1)."""
+        if x_init is None:
+            if strength != 1:
+                raise ValueError(f"strength={strength} needs x_init (sampling from pure noise is strength 1)")
+            return 0
+        k0 = self.start_step(len(self.ddim_timesteps), strength)
+        shape, got = tuple(shape), tuple(x_init.shape)
+        if len(got) != 4 or got[0] not in (1, shape[0]) or got[1:] != shape[1:]:
+            raise ValueError(f"x_init of shape {got} does not fit the latent {shape} (want (1 or B, C, H, W))")
+        return k0
+
+    def start_latent(self, shape, x_init: torch.Tensor, k0: int) -> torch.Tensor:
+        """x_start = sqrt(acp[t0]) * x_init + sqrt(1 - acp[t0]) * z at t0 = time_range[k0], z keyed by `self.seed`
+        (ops.noise_latent), x_init broadcast over the batch of `shape`."""
+        t0 = int(np.flip(self.ddim_timesteps)[k0])
+        a = float(self.alphas_cumprod[t0])
+        x = torch.empty(tuple(shape), dtype=torch.float32, device=self.device)
+        ops.noise_latent(x_init.to(device=self.device, dtype=torch.float32).contiguous(), a, self.seed, x)
+        return x
+
+    def init_run(self, shape, x_init, strength, seed, noisy=False) -> Tuple[int, Optional[torch.Tensor]]:
+        """A sampler's image-to-image set-up: validates, sets `self.seed` (`resolve_seed`: a run draws noise when it
+        has x_init or `noisy` says so) and returns (k0, x_start), x_start None without x_init."""
+        k0 = self.check_init(shape, x_init, strength)
+        self.seed = resolve_seed(noisy or x_init is not None, seed)
+        return k0, None if x_init is None else self.start_latent(shape, x_init, k0)

@@ -9,7 +9,9 @@ PLMS updates are `PLMSBase._step_predict` / `_step_finish` on its own trajectori
 and a Multi-instance request merges its latents with `ops.latent_mean` at its own step int(steps * mis), where
 steps is the length of the PLMS schedule (`schedule_steps`: S + 1 for some S, e.g. 31 for S = 30), as there.
 A DDIM request (`sampler="ddim"`) takes `DDIMBase`'s one-evaluation update instead, its eta noise keyed by its own seed
-and the step, so it does not depend on the other requests.  That per-request machinery is `_RequestState`, which
+and the step, so it does not depend on the other requests.  An image-to-image request (`x_init`, `strength`) starts at
+its sampler's step k0 from x_init noised there (`PLMSBase.start_latent`); in lock step it joins the others at step k0,
+so every request ends with the last step.  That per-request machinery is `_RequestState`, which
 `SamplingEngine` (engine.py) drives too: `sample_requests` is the lock-step driver on top of it.
 
 Contract: each returned latent equals, within floating-point tolerance, what `PLMSSampler.sample()` (input dict,
@@ -29,8 +31,8 @@ import torch
 from .... import ops
 from ...modules.attention import GatedSelfAttentionDense
 from ...modules.diffusionmodules.util import make_ddim_timesteps
-from ._plms_common import PLMSBase, Trajectory
-from .ddim import DDIMBase, resolve_seed
+from ._plms_common import PLMSBase, Trajectory, resolve_seed
+from .ddim import DDIMBase
 
 
 @dataclass
@@ -41,7 +43,9 @@ class Request:
     from the call (S, if given, must equal it), `SamplingEngine` requires it.  `mask` / `x0` (inpainting) are not
     supported and raise.  `sampler`: "plms", or "ddim" (`DDIMSampler.sample`: input dict only) with its `eta` and
     `seed` (None at eta > 0: one draw from torch's default CPU generator when `sample_requests` starts or at `submit`,
-    in request order)."""
+    in request order).  `x_init`: a latent of shape (1 or B, C, H, W) to start image-to-image sampling from, which
+    runs the last int(N * strength) of the N schedule steps (the samplers' `x_init` / `strength`); the start noise is
+    keyed by `seed`, drawn as for DDIM when None."""
     input: Union[dict, List[dict]]
     uc: Optional[torch.Tensor] = None
     guidance_scale: float = 1.0
@@ -54,6 +58,8 @@ class Request:
     sampler: str = "plms"
     eta: float = 0.0
     seed: Optional[int] = None
+    x_init: Optional[torch.Tensor] = None
+    strength: float = 1.0
 
 
 SAMPLERS = ("plms", "ddim")
@@ -62,14 +68,18 @@ SAMPLERS = ("plms", "ddim")
 @dataclass(frozen=True)
 class RequestPlan:
     """What the step planner needs of a request: trajectories before the merge (1 for plain PLMS), the step
-    before which they merge (None: never), images per trajectory and whether it evaluates cond + uncond."""
+    before which they merge (None: never), images per trajectory, whether it evaluates cond + uncond and the step it
+    starts at (k0 > 0: image-to-image)."""
     trajectories: int
     merge_step: Optional[int]
     images: int
     cfg: bool
+    k0: int = 0
 
     def live(self, step: int) -> int:
         """Trajectories evaluated at `step`."""
+        if step < self.k0:
+            return 0
         return self.trajectories if self.merge_step is not None and step < self.merge_step else 1
 
     def rows(self) -> int:
@@ -113,7 +123,8 @@ def schedule_steps(S: int, ddpm_timesteps: int = 1000) -> int:
 def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_timesteps: int = 1000) -> List[RequestPlan]:
     """Validate the requests of one `sample_requests` call and describe them for the planner.  All must share the
     step count S, the latent height x width and the context length; mask / x0 inpainting is not supported.
-    A Multi-instance request merges before step int(schedule_steps(S) * mis), as PLMSSamplerInst does."""
+    A Multi-instance request merges before step int(schedule_steps(S) * mis), as PLMSSamplerInst does (an
+    image-to-image one only if that step lies after its start step k0, `PLMSBase.mis_merge_step`)."""
     if not 0 < int(S) <= int(ddpm_timesteps):
         raise ValueError(f"S must be in [1, {ddpm_timesteps}], got {S}")
     steps = schedule_steps(S, ddpm_timesteps)
@@ -164,8 +175,22 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
                 ctx_len = t.shape[1]
             elif t.shape[1] != ctx_len:
                 raise ValueError(f"request {j}: context length {t.shape[1]} differs from {ctx_len}")
+        k0 = 0
+        if req.x_init is None:
+            if req.strength != 1:
+                raise ValueError(f"request {j}: strength={req.strength} needs x_init")
+        else:
+            try:
+                k0 = PLMSBase.start_step(steps, req.strength)
+            except ValueError as e:
+                raise ValueError(f"request {j}: {e}") from None
+            xs = tuple(req.x_init.shape)
+            if len(xs) != 4 or xs[0] not in (1, shape[0]) or xs[1:] != shape[1:]:
+                raise ValueError(f"request {j}: x_init of shape {xs} does not fit the latent {shape} "
+                                 "(want (1 or B, C, H, W))")
         cfg = req.uc is not None and req.guidance_scale != 1
-        plans.append(RequestPlan(len(ins), int(steps * req.mis) if multi else None, shape[0], cfg))
+        merge = PLMSBase.mis_merge_step(steps, req.mis, k0, req.x_init is not None) if multi else None
+        plans.append(RequestPlan(len(ins) if merge is not None else 1, merge, shape[0], cfg, k0))
     return plans
 
 
@@ -181,10 +206,11 @@ class _RequestState:
         if req.sampler == "ddim":
             self.base = DDIMBase(diffusion, model)
             self.base.make_schedule(ddim_num_steps=int(S), ddim_eta=float(req.eta))
-            self.base.seed = resolve_seed(self.base.ddim_eta, req.seed)
         else:
             self.base = PLMSBase(diffusion, model)
             self.base.make_schedule(ddim_num_steps=int(S))
+        noisy = req.sampler == "ddim" and self.base.ddim_eta > 0
+        self.base.seed = resolve_seed(noisy or req.x_init is not None, req.seed)
         self.time_range = np.flip(self.base.ddim_timesteps)
         self.steps = len(self.time_range)
         self.alphas = req.alpha_generator_func(self.steps) if req.alpha_generator_func is not None else None
@@ -203,22 +229,30 @@ class _RequestState:
         self.null_input = None if own else gti.get_null_input(batch=plan.images)
         ins = _inputs_of(req)
         x = next((i["x"] for i in ins if i.get("x") is not None), None)
-        self.group = (tuple(x.shape[2:]) if x is not None else tuple(req.shape[2:]), ins[0]["context"].shape[1])
+        self.shape = tuple(x.shape) if x is not None else tuple(req.shape)
+        self.group = (self.shape[2:], ins[0]["context"].shape[1])
         self.trajs: List[Trajectory] = []
         self.gs = float(req.guidance_scale)
         self.reached_zero = False
-        self.i = 0             # current step
+        self.i = plan.k0       # current step
         self.pending = None    # predictor state while the corrector's evaluation is due
         self.ts_next = None
 
     def start(self):
-        """The trajectories, when the request starts sampling."""
+        """The trajectories, when the request starts sampling: an image-to-image request's start latent is made here,
+        before its first forward."""
         ins = _inputs_of(self.req)
-        if ins[0].get("x") is None:  # as the samplers: one noise tensor shared by every trajectory
-            img = torch.randn(tuple(self.req.shape), device=self.base.device)
+        if self.req.x_init is not None:
+            img = self.base.start_latent(self.shape, self.req.x_init, self.plan.k0)
+        elif ins[0].get("x") is None:  # as the samplers: one noise tensor shared by every trajectory
+            img = torch.randn(self.shape, device=self.base.device)
+        else:
+            img = None
+        if img is not None:
             for inp in ins:
                 inp["x"] = img
-        self.trajs = [Trajectory(inp) for inp in ins]
+        # a Multi-instance image-to-image request whose merge falls before its start runs the global trajectory alone
+        self.trajs = [Trajectory(inp) for inp in ins[:self.plan.trajectories]]
 
     def images(self) -> int:
         """Images the request puts into an evaluation before its merge."""
@@ -365,21 +399,29 @@ def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], 
         st.start()
     steps = states[0].steps
     # the model's hoisted-tensor caches must hold every input and every chunk combination of the run, or each
-    # forward recomputes its text / object K/V: raised for the run
+    # forward recomputes its text / object K/V: raised for the run.  Image-to-image PLMS requests take the corrector's
+    # evaluation of their first step in forwards of their own at their start step.
     chunks = {tuple(c) for i in range(steps) for c in plan_step(plans, i, max_batch)}
+    for k0 in {p.k0 for p in plans if p.k0 > 0}:
+        slots = [(r, k) for r, p in enumerate(plans) if p.k0 == k0 and reqs[r].sampler == "plms"
+                 for k in range(p.live(k0))]
+        chunks |= {tuple(c) for c in plan_chunks(slots, plans, max_batch)}
     try:
         with _RequestState.cache_bounds(model, sum(p.trajectories + 2 for p in plans) + 8, 2 * len(chunks) + 2):
-            for _ in range(steps):
-                scales = []
-                for st in states:
+            for step in range(steps):
+                live = [r for r, p in enumerate(plans) if p.k0 <= step]  # image-to-image requests join at k0
+                scales, flags = [0.0] * len(states), [False] * len(states)
+                for r in live:
+                    st = states[r]
                     st.begin()
                     zero = st.reached_zero
-                    scales.append(st.fuser_scale())
+                    scales[r] = st.fuser_scale()
                     if st.reached_zero and not zero:
                         model.restore_first_conv_from_SD()  # the swap a run of this request makes here
                 sd_conv = bool(getattr(model, "_first_conv_restored", False))
-                flags = [st.conv_flag(sd_conv) for st in states]
-                todo = range(len(states))
+                for r in live:
+                    flags[r] = states[r].conv_flag(sd_conv)
+                todo = live
                 while todo:  # every request's step, then the corrector's evaluation of a first PLMS step
                     slots = [(r, k) for r in todo for k in range(len(states[r].trajs))]
                     forwards = [(c, None) for c in plan_chunks(slots, plans, max_batch)]

@@ -25,27 +25,12 @@ import torch
 
 from .... import ops
 from ...modules.diffusionmodules.util import make_ddim_sampling_parameters
-from ._plms_common import PLMSBase, Trajectory
-
-
-def resolve_seed(eta: float, seed: Optional[int]) -> int:
-    """The seed of a DDIM run: `seed` if given; at eta > 0 otherwise one draw from torch's default CPU generator;
-    0 at eta = 0, where no noise is drawn (the generator is left untouched)."""
-    if seed is not None:
-        seed = int(seed)
-        if not 0 <= seed < 1 << 64:
-            raise ValueError(f"seed {seed} outside [0, 2^64)")
-        return seed
-    if eta == 0:
-        return 0
-    return int(torch.randint(0, 2 ** 63 - 1, (1,), dtype=torch.int64).item())
+from ._plms_common import PLMSBase, Trajectory, resolve_seed  # noqa: F401 (resolve_seed: batched.py)
 
 
 class DDIMBase(PLMSBase):
     """`PLMSBase` with the DDIM update: `make_schedule` keeps the eta sigmas, `_step_predict` has nothing to predict and
     `_step_finish` is one `ops.ddim_update` per trajectory, its noise keyed by (`self.seed`, index)."""
-
-    seed = 0
 
     def make_schedule(self, ddim_num_steps, ddim_discretize="uniform", ddim_eta=0., verbose=False):
         """ddim.py:25-54: the schedule of `PLMSBase.make_schedule` and the sigmas of `ddim_eta` (util.py:73-83)."""
@@ -78,19 +63,23 @@ class DDIMSampler(DDIMBase):
         super().__init__(diffusion, model, schedule, alpha_generator_func, set_alpha_scale)
 
     @torch.no_grad()
-    def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, eta=0.0, seed=None):
+    def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, eta=0.0, seed=None,
+               x_init=None, strength=1.0):
         """ddim.py:57-60.  `input` is one input dict (there is no Multi-instance DDIM sampler).  eta > 0 adds the
-        stochastic term of DDIM, its noise fixed by `seed` (see the module docstring)."""
+        stochastic term of DDIM, its noise fixed by `seed` (see the module docstring).  x_init / strength start
+        image-to-image sampling as in PLMSSampler.sample; `seed` keys that start noise too."""
         if not isinstance(input, dict):
             raise ValueError("DDIMSampler.sample takes one input dict; the Multi-instance input list is PLMS only "
                              "(PLMSSamplerInst)")
         self.make_schedule(ddim_num_steps=S, ddim_eta=eta)
-        self.seed = resolve_seed(self.ddim_eta, seed)
-        return self.ddim_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0)
+        k0, x_start = self.init_run(shape, x_init, strength, seed, noisy=self.ddim_eta > 0)
+        if x_start is not None:
+            input["x"] = x_start
+        return self.ddim_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0, k0=k0)
 
     @torch.no_grad()
-    def ddim_sampling(self, shape, input, uc, guidance_scale=1, mask=None, x0=None):
-        """ddim.py:63-103."""
+    def ddim_sampling(self, shape, input, uc, guidance_scale=1, mask=None, x0=None, k0=0):
+        """ddim.py:63-103, from step k0 (image-to-image) on."""
         b = shape[0]
         if input["x"] is None:
             input["x"] = torch.randn(shape, device=self.device)
@@ -98,7 +87,7 @@ class DDIMSampler(DDIMBase):
         total_steps = self.ddim_timesteps.shape[0]
         alphas = self.alpha_generator_func(len(time_range)) if self.alpha_generator_func is not None else None
         tr = Trajectory(input)
-        for i in range(len(time_range)):
+        for i in range(k0, len(time_range)):
             if alphas is not None:
                 self._set_alpha(alphas[i])
             ts, ts_next = self._timesteps(b, i, time_range)

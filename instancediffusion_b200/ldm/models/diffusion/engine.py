@@ -14,8 +14,10 @@ next tick with everyone else).  A PLMS request therefore retires after schedule_
 (one evaluation per step) after schedule_steps(S).  Each request is a `batched._RequestState`, the per-request sampling
 state that `sample_requests` drives too: its own schedule (`make_schedule(S)` of `PLMSBase`, or of `DDIMBase` with its
 eta and seed), its sampler's arithmetic (`_step_predict` / `_step_finish`) and its Multi-instance merge before step
-int(schedule_steps(S) * mis), after the last one for mis = 1.  PLMS and DDIM requests of one latent size and context
-length share forwards.  The engine adds admission, the grouping of a tick's forwards and retirement.
+int(schedule_steps(S) * mis), after the last one for mis = 1.  An image-to-image request (`x_init`, `strength`) starts
+at its step k0 with the start latent made at admission, before its first forward, and so retires after n_run =
+schedule_steps(S) - k0 ticks (DDIM) or n_run + 1 (PLMS).  PLMS and DDIM requests of one latent size and context
+length, and of any strength, share forwards.  The engine adds admission, the grouping of a tick's forwards and retirement.
 
 The evaluations of a tick are grouped by (latent H x W, context length) in admission order, split into forwards of
 at most `max_batch` images by `plan_chunks`, and each forward is padded to the smallest of `buckets` that holds it.

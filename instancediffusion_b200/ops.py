@@ -7,6 +7,7 @@ tensor without synchronising.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Optional, Tuple
 
 import torch
@@ -504,6 +505,30 @@ def ddim_update(x: torch.Tensor, e_c: torch.Tensor, e_u: Optional[torch.Tensor],
     check(lib.idiff_ddim_update(x.data_ptr(), e_c.data_ptr(), _ptr(e_u), float(gs), float(a_t), float(a_prev),
                                 float(sigma), seed, int(index), _ptr(e_out), x_out.data_ptr(), x.numel(), _stream()),
           "idiff_ddim_update")
+
+
+def noise_latent(x_init: torch.Tensor, a: float, seed: int, out: torch.Tensor) -> torch.Tensor:
+    """The image-to-image start latent (include/idiff_b200.h idiff_noise_latent): out = sqrt(a) * x_init + sqrt(1 - a)
+    * z, x_init broadcast over out's leading elements (out.numel() a multiple of x_init.numel()), z a function of (seed,
+    element) only.  a: alphas_cumprod at the start timestep, in [0, 1]; the two square roots are taken in float64 and
+    rounded to fp32.  fp32 contiguous tensors; seed: an integer in [0, 2^64)."""
+    lib = _lib.load()
+    for name, t in (("x_init", x_init), ("out", out)):
+        _req(t, torch.float32, name)
+        if not t.is_contiguous() or t.numel() == 0:
+            raise _lib.IdiffError(f"noise_latent: {name} must be contiguous and non-empty")
+    if out.numel() % x_init.numel():
+        raise _lib.IdiffError(f"noise_latent: out has {out.numel()} elements, not a multiple of x_init's "
+                              f"{x_init.numel()}")
+    a = float(a)
+    if not 0.0 <= a <= 1.0:
+        raise _lib.IdiffError(f"noise_latent: a={a} outside [0, 1]")
+    seed = int(seed)
+    if not 0 <= seed < 1 << 64:
+        raise _lib.IdiffError(f"noise_latent: seed {seed} outside [0, 2^64)")
+    check(lib.idiff_noise_latent(x_init.data_ptr(), x_init.numel(), math.sqrt(a), math.sqrt(1.0 - a), seed,
+                                 out.data_ptr(), out.numel(), _stream()), "idiff_noise_latent")
+    return out
 
 
 def latent_mean(xs, out: torch.Tensor) -> torch.Tensor:
