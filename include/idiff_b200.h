@@ -317,6 +317,12 @@ int idiff_vae_latent_in(const float* z, const float* w, const float* bias, float
 /* in-place softmax over the n columns of each of `rows` fp16 rows (row stride ld elements), fp32 arithmetic:
    the attention weights of AttnBlock (model.py:185-187); the 1/sqrt(c) scale is folded into the q projection */
 int idiff_softmax_rows(void* x, int rows, int n, long ld, void* stream);
+/* inference.py:122-125, the image a request's latent stands for: the decoder's output x (batch, 3, hw) NCHW, fp32
+   (x_fp32 = 1, what AutoencoderKL.decode returns) or the 16-bit storage type (x_fp32 = 0), to uint8 NHWC
+   out[batch][hw][3] = (uint8)((min(max(x, -1), 1) * 0.5 + 0.5) * 255) in fp32, truncated toward zero like numpy's
+   astype(np.uint8); +-inf clamp to 0 / 255 and NaN gives 0.  Any hw; hw % 4 == 0 with x 16-byte (fp32) / 8-byte
+   (16-bit) and out 4-byte aligned takes vector loads and stores. */
+int idiff_decode_to_image(const void* x, int x_fp32, void* out, int batch, long hw, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * CLIP text encoder (host prep, SURVEY.md section 8f-3): the per-phrase pooled feature of

@@ -92,6 +92,7 @@ SIGNATURES = {
     "idiff_attmask_words": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "idiff_vae_latent_in": (_i, [_vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp]),
     "idiff_softmax_rows": (_i, [_vp, _i, _i, _l, _vp]),
+    "idiff_decode_to_image": (_i, [_vp, _i, _vp, _i, _l, _vp]),
     "idiff_embed_tokens": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "idiff_causal_attention_small": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
 }

@@ -4,7 +4,8 @@
 //     the 64-channel granularity of the conv3x3 kernel's A operand;
 //   * row softmax of the single-head mid-block attention (AttnBlock, model.py:150-202): the scores of one
 //     image are a [HW, HW] GEMM output (head_dim 512 does not fit the flash kernels' register tiles and the
-//     block runs once per image), normalised in place.
+//     block runs once per image), normalised in place;
+//   * image epilogue: the decoder's NCHW output to the uint8 NHWC bytes the reference saves (inference.py:122-125).
 #include "../../include/idiff_b200.h"
 #include "common.cuh"
 #include "host.cuh"
@@ -102,6 +103,66 @@ softmax_rows_kernel(h16* __restrict__ x, int n, long ld) {
   }
 }
 
+// inference.py:122-125 for one value: torch.clamp(x, -1, 1) * 0.5 + 0.5 on the device, then * 255 and
+// astype(np.uint8) in numpy, all fp32.  x * 0.5 is exact, so one fma rounds like the reference's mul + add; the
+// conversion truncates toward zero like the C cast numpy uses.  NaN clamps to -1 (fmaxf returns the other operand).
+IDIFF_DEVICE uint32_t image_byte(float x) {
+  const float c = fminf(fmaxf(x, -1.f), 1.f);
+  return __float2uint_rz(__fmul_rn(__fmaf_rn(c, 0.5f, 0.5f), 255.f));
+}
+
+IDIFF_DEVICE float load_f(const float* p) { return *p; }
+IDIFF_DEVICE float load_f(const h16* p) { return h2f(*p); }
+
+// four consecutive pixels of one channel plane: one 16-byte (fp32) or 8-byte (16-bit) load
+IDIFF_DEVICE void load4(const float* p, float v[4]) {
+  const float4 u = *reinterpret_cast<const float4*>(p);
+  v[0] = u.x, v[1] = u.y, v[2] = u.z, v[3] = u.w;
+}
+IDIFF_DEVICE void load4(const h16* p, float v[4]) {
+  const uint2 u = *reinterpret_cast<const uint2*>(p);
+  const float2 a = unpack_half2(u.x), b = unpack_half2(u.y);
+  v[0] = a.x, v[1] = a.y, v[2] = b.x, v[3] = b.y;
+}
+
+// One thread per group of four pixels of one image: the three channel planes in (NCHW), the 12 bytes of those pixels
+// out (NHWC), which are three aligned 32-bit words.  VEC (HW % 4 == 0): every group is whole and its loads and stores
+// are aligned; otherwise the last group of an image may be partial and everything goes element by element.
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(256)
+decode_to_image_kernel(const T* __restrict__ x, uint8_t* __restrict__ out, int B, long HW) {
+  constexpr int C = 3;
+  pdl_launch_dependents();
+  pdl_wait();
+  const long groups = (HW + 3) / 4;
+  const long total = (long)B * groups;
+  for (long g = (long)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long b = g / groups;
+    const long p0 = (g - b * groups) * 4;
+    const T* src = x + b * C * HW + p0;
+    uint8_t* dst = out + (b * HW + p0) * C;
+    if (VEC) {
+      uint32_t w[C] = {0u, 0u, 0u};  // byte k of the group's output is channel k % 3 of pixel k / 3
+#pragma unroll
+      for (int c = 0; c < C; ++c) {
+        float v[4];
+        load4(src + c * HW, v);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int k = j * C + c;
+          w[k >> 2] |= image_byte(v[j]) << (8 * (k & 3));
+        }
+      }
+#pragma unroll
+      for (int q = 0; q < C; ++q) reinterpret_cast<uint32_t*>(dst)[q] = w[q];
+    } else {
+      const int n = (int)(HW - p0 < 4 ? HW - p0 : 4);
+      for (int j = 0; j < n; ++j)
+        for (int c = 0; c < C; ++c) dst[j * C + c] = (uint8_t)image_byte(load_f(src + c * HW + j));
+    }
+  }
+}
+
 }  // namespace idiff
 
 extern "C" int idiff_vae_latent_in(const float* z, const float* w, const float* bias, float inv_scale, void* out,
@@ -130,6 +191,28 @@ extern "C" int idiff_softmax_rows(void* x, int rows, int n, long ld, void* strea
   }
   IDIFF_CHECK_CUDA(launch_pdl(softmax_rows_kernel, dim3(rows), dim3(256), smem, reinterpret_cast<cudaStream_t>(stream),
                               reinterpret_cast<h16*>(x), n, ld));
+  IDIFF_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int idiff_decode_to_image(const void* x, int x_fp32, void* out, int batch, long hw, void* stream) {
+  using namespace idiff;
+  IDIFF_REQUIRE(x && out && batch > 0 && hw > 0, "idiff_decode_to_image: bad arguments");
+  const bool vec = hw % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & (x_fp32 ? 15 : 7)) == 0 &&
+                   (reinterpret_cast<uintptr_t>(out) & 3) == 0;
+  const long total = (long)batch * ((hw + 3) / 4);
+  const int blocks = (int)((total + 255) / 256 < num_sms() * 16 ? (total + 255) / 256 : num_sms() * 16);
+  const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  uint8_t* o = reinterpret_cast<uint8_t*>(out);
+  if (x_fp32) {
+    const float* xf = reinterpret_cast<const float*>(x);
+    IDIFF_CHECK_CUDA(vec ? launch_pdl(decode_to_image_kernel<float, true>, dim3(blocks), dim3(256), 0, s, xf, o, batch, hw)
+                         : launch_pdl(decode_to_image_kernel<float, false>, dim3(blocks), dim3(256), 0, s, xf, o, batch, hw));
+  } else {
+    const h16* xh = reinterpret_cast<const h16*>(x);
+    IDIFF_CHECK_CUDA(vec ? launch_pdl(decode_to_image_kernel<h16, true>, dim3(blocks), dim3(256), 0, s, xh, o, batch, hw)
+                         : launch_pdl(decode_to_image_kernel<h16, false>, dim3(blocks), dim3(256), 0, s, xh, o, batch, hw));
+  }
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

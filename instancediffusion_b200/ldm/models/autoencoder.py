@@ -69,3 +69,11 @@ class AutoencoderKL(PackedModule):
         B, _, H, W = z.shape
         z16 = ops.vae_latent_in(z.float().contiguous(), p["wpq"], p["bpq"], 1.0 / float(self.scale_factor))
         return self.decoder._decode_tokens(z16, B, H, W)
+
+    @torch.no_grad()
+    def decode_images(self, z):
+        """z (B, 4, h, w) -> uint8 (B, 8h, 8w, 3) on the device: `decode(z)` and the bytes inference.py:122-125 saves
+        (clamp to [-1, 1], * 0.5 + 0.5, * 255, truncated like astype(np.uint8)) in one kernel."""
+        x = self.decode(z)
+        B, _, H, W = x.shape
+        return ops.decode_to_image(x, torch.empty((B, H, W, 3), dtype=torch.uint8, device=x.device))

@@ -12,7 +12,9 @@ A DDIM request (`sampler="ddim"`) takes `DDIMBase`'s one-evaluation update inste
 and the step, so it does not depend on the other requests.  An image-to-image request (`x_init`, `strength`) starts at
 its sampler's step k0 from x_init noised there (`PLMSBase.start_latent`); in lock step it joins the others at step k0,
 so every request ends with the last step.  That per-request machinery is `_RequestState`, which
-`SamplingEngine` (engine.py) drives too: `sample_requests` is the lock-step driver on top of it.
+`SamplingEngine` (engine.py) drives too: `sample_requests` is the lock-step driver on top of it.  A request with
+`output="image"` gets the image of its latent instead: the drivers decode the latents of the image requests that finish
+together in batched first-stage forwards (`decode_latents`), eagerly and apart from the UNet's caches and graphs.
 
 Contract: each returned latent equals, within floating-point tolerance, what `PLMSSampler.sample()` (input dict,
 mis = 0), `PLMSSamplerInst.sample()` (input list [global, instance_1 .. instance_n]) or `DDIMSampler.sample(eta=,
@@ -45,7 +47,8 @@ class Request:
     `seed` (None at eta > 0: one draw from torch's default CPU generator when `sample_requests` starts or at `submit`,
     in request order).  `x_init`: a latent of shape (1 or B, C, H, W) to start image-to-image sampling from, which
     runs the last int(N * strength) of the N schedule steps (the samplers' `x_init` / `strength`); the start noise is
-    keyed by `seed`, drawn as for DDIM when None."""
+    keyed by `seed`, drawn as for DDIM when None.  `output`: "latent" (the sampler's latent) or "image" (that latent
+    decoded by the driver's `autoencoder` to uint8 (B, 8H, 8W, 3) on the device, `AutoencoderKL.decode_images`)."""
     input: Union[dict, List[dict]]
     uc: Optional[torch.Tensor] = None
     guidance_scale: float = 1.0
@@ -60,9 +63,11 @@ class Request:
     seed: Optional[int] = None
     x_init: Optional[torch.Tensor] = None
     strength: float = 1.0
+    output: str = "latent"
 
 
 SAMPLERS = ("plms", "ddim")
+OUTPUTS = ("latent", "image")
 
 
 @dataclass(frozen=True)
@@ -141,6 +146,8 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
         multi = isinstance(req.input, (list, tuple))
         if req.sampler not in SAMPLERS:
             raise ValueError(f"request {j}: unknown sampler {req.sampler!r} (have {', '.join(SAMPLERS)})")
+        if req.output not in OUTPUTS:
+            raise ValueError(f"request {j}: unknown output {req.output!r} (have {', '.join(OUTPUTS)})")
         if not req.eta >= 0:
             raise ValueError(f"request {j}: eta={req.eta} must be >= 0")
         if req.sampler == "plms" and req.eta != 0:
@@ -380,11 +387,44 @@ class _RequestState:
                     delattr(model, k)
 
 
+def check_decode(requests: Sequence[Request], autoencoder, max_decode_batch: int) -> None:
+    """The decode settings of a driver for `requests`: image requests need an autoencoder."""
+    if int(max_decode_batch) <= 0:
+        raise ValueError(f"max_decode_batch must be positive, got {max_decode_batch}")
+    if autoencoder is None:
+        for j, req in enumerate(requests):
+            if req.output == "image":
+                raise ValueError(f"request {j}: output='image' needs the driver's autoencoder (autoencoder=None)")
+
+
+def decode_latents(autoencoder, latents: Sequence[torch.Tensor], max_decode_batch: int) -> List[torch.Tensor]:
+    """The images of `latents` (each (B_j, 4, h, w)), decoded together: the latents of one size are concatenated in
+    order and run through `autoencoder.decode_images` in chunks of at most `max_decode_batch` images; one uint8
+    (B_j, 8h, 8w, 3) tensor per latent, in order."""
+    out: List[Optional[torch.Tensor]] = [None] * len(latents)
+    by_size: Dict[tuple, List[int]] = {}
+    for j, z in enumerate(latents):
+        by_size.setdefault(tuple(z.shape[1:]), []).append(j)
+    m = int(max_decode_batch)
+    for js in by_size.values():
+        z = latents[js[0]] if len(js) == 1 else torch.cat([latents[j] for j in js])
+        parts = [autoencoder.decode_images(z[s:s + m]) for s in range(0, z.shape[0], m)]
+        imgs = parts[0] if len(parts) == 1 else torch.cat(parts)
+        start = 0
+        for j in js:
+            out[j] = imgs[start:start + latents[j].shape[0]]
+            start += latents[j].shape[0]
+    return out
+
+
 @torch.no_grad()
 def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], S: int, *,
-                    max_batch: int = 32) -> List[torch.Tensor]:
+                    max_batch: int = 32, autoencoder=None, max_decode_batch: int = 8) -> List[torch.Tensor]:
     """Sample every request in `requests` (Request objects or dicts of its fields) with S steps of its sampler; returns
-    one latent per request, in order.  `max_batch` bounds the images of one UNet forward.
+    one latent per request, in order, or for an `output="image"` request its uint8 (B, 8H, 8W, 3) image.  `max_batch`
+    bounds the images of one UNet forward.  After the last step the latents of the image requests are decoded
+    together by `autoencoder` (an `AutoencoderKL`, required when a request asks for an image), at most
+    `max_decode_batch` images per decoder forward (`decode_latents`).
 
     The per-image fuser scales are those `utils.model.set_alpha_scale` sets (every gated fuser at the request's
     alpha), and the model is left with that function's result for the last alpha of the last request that has an
@@ -394,6 +434,7 @@ def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], 
     from ....utils.model import set_alpha_scale
     reqs = [r if isinstance(r, Request) else Request(**r) for r in requests]
     plans = check_requests(reqs, S, max_batch, diffusion.num_timesteps)
+    check_decode(reqs, autoencoder, max_decode_batch)
     states = [_RequestState(r, p, S, model, diffusion) for r, p in zip(reqs, plans)]
     for st in states:
         st.start()
@@ -437,4 +478,8 @@ def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], 
         if st.alphas is not None:
             set_alpha_scale(model, st.alphas[-1])
             break
+    images = [j for j, r in enumerate(reqs) if r.output == "image"]
+    if images:
+        for j, img in zip(images, decode_latents(autoencoder, [latents[j] for j in images], max_decode_batch)):
+            latents[j] = img
     return latents

@@ -8,6 +8,10 @@ when the slowest one finishes.  `SamplingEngine` lets requests join and leave be
     done = engine.step()                 # one tick: {ticket: latent} of the requests that finished in it
     done = engine.drain()                # tick until nothing is queued or live
 
+A request with `output="image"` (the engine built with `autoencoder=`) finishes with its uint8 (B, 8H, 8W, 3) image
+instead of its latent: the image requests that finish in a tick are decoded together in that tick, at most
+`max_decode_batch` images per first-stage forward (`batched.decode_latents`), eagerly, outside the UNet's graphs.
+
 A tick gives every live trajectory exactly one UNet evaluation: the one at t of its current step or, for a request
 in the Euler predictor of its first PLMS step, the corrector's evaluation at t_next (so the corrector rides in the
 next tick with everyone else).  A PLMS request therefore retires after schedule_steps(S) + 1 ticks, a DDIM request
@@ -37,7 +41,7 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 
-from .batched import Request, RequestPlan, _RequestState, check_requests, plan_chunks
+from .batched import Request, RequestPlan, _RequestState, check_decode, check_requests, decode_latents, plan_chunks
 
 
 def pick_bucket(images: int, unit: int, buckets: Optional[Sequence[int]]) -> Optional[int]:
@@ -69,12 +73,16 @@ class SamplingEngine:
     """Step-level scheduler of sampling requests on one model.  `max_batch`: images per UNet forward;
     `max_live_images`: bound of the images of the admitted requests (default 4 * max_batch); `buckets`: the padded
     forward sizes (None: no padding); `share_graph_pool`: capture the graphs of the engine's forwards into one
-    memory pool instead of a private pool each (see README)."""
+    memory pool instead of a private pool each (see README); `autoencoder`: the `AutoencoderKL` that decodes
+    `output="image"` requests, at most `max_decode_batch` images per decoder forward."""
 
     def __init__(self, model, diffusion, *, max_batch: int = 32, max_live_images: Optional[int] = None,
-                 buckets: Optional[Sequence[int]] = (2, 4, 8, 16, 24, 32), share_graph_pool: bool = False):
+                 buckets: Optional[Sequence[int]] = (2, 4, 8, 16, 24, 32), share_graph_pool: bool = False,
+                 autoencoder=None, max_decode_batch: int = 8):
         if int(max_batch) <= 0:
             raise ValueError(f"max_batch must be positive, got {max_batch}")
+        check_decode([], autoencoder, max_decode_batch)
+        self.autoencoder, self.max_decode_batch = autoencoder, int(max_decode_batch)
         self.model, self.diffusion = model, diffusion
         self.max_batch = int(max_batch)
         self.max_live_images = 4 * self.max_batch if max_live_images is None else int(max_live_images)
@@ -110,6 +118,7 @@ class SamplingEngine:
         if req.S is None:
             raise ValueError("request.S (the request's step count) is required")
         plan = check_requests([req], int(req.S), self.max_batch, self.diffusion.num_timesteps)[0]
+        check_decode([req], self.autoencoder, self.max_decode_batch)
         size = plan.trajectories * plan.rows()
         if size > self.max_live_images:
             raise ValueError(f"request of {size} images (trajectories x images x CFG) exceeds max_live_images="
@@ -120,7 +129,7 @@ class SamplingEngine:
         return ticket
 
     def drain(self) -> Dict[int, torch.Tensor]:
-        """Tick until nothing is queued or live; the latents of every request that finished meanwhile."""
+        """Tick until nothing is queued or live; the latents (images) of every request that finished meanwhile."""
         done = {}
         while self._queue or self._live:
             done.update(self.step())
@@ -128,7 +137,8 @@ class SamplingEngine:
 
     @torch.no_grad()
     def step(self) -> Dict[int, torch.Tensor]:
-        """One tick: admit, evaluate every live trajectory once, advance; {ticket: latent} of the finished requests."""
+        """One tick: admit, evaluate every live trajectory once, advance; {ticket: latent} of the finished requests
+        ({ticket: image} for image requests, decoded together after the tick's forwards)."""
         live_images = sum(st.images() for st in self._live.values())
         while self._queue and live_images + self._queue[0][1].images() <= self.max_live_images:
             ticket, st = self._queue.popleft()
@@ -158,6 +168,11 @@ class SamplingEngine:
         if finished:
             keep = [i for st in list(self._live.values()) + [st for _, st in self._queue] for i in st.inputs()]
             self.model.drop_hoisted([i for st in finished for i in st.inputs()], keep)
+        images = [t for t, st in zip(done, finished) if st.req.output == "image"]
+        if images:
+            for t, img in zip(images, decode_latents(self.autoencoder, [done[t] for t in images],
+                                                     self.max_decode_batch)):
+                done[t] = img
         return done
 
     def _run(self, states, forwards, scales, flags):

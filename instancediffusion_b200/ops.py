@@ -664,6 +664,29 @@ def softmax_rows_(x: torch.Tensor) -> torch.Tensor:
     return x
 
 
+def decode_to_image(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """The decoder's image to the bytes the reference saves (include/idiff_b200.h idiff_decode_to_image): x (B, 3, H, W)
+    fp32 or the 16-bit storage type, contiguous NCHW -> out uint8 (B, H, W, 3) contiguous, out = trunc((clamp(x, -1, 1)
+    * 0.5 + 0.5) * 255) in fp32."""
+    lib = _lib.load()
+    if x.dtype not in (torch.float32, HALF):
+        raise _lib.IdiffError(f"decode_to_image: x must be torch.float32 or {HALF}, got {x.dtype}")
+    _req(x, x.dtype, "x")
+    _req(out, torch.uint8, "out")
+    if x.dim() != 4 or x.shape[1] != 3 or x.numel() == 0 or not x.is_contiguous():
+        raise _lib.IdiffError(f"decode_to_image: x must be a contiguous non-empty (B, 3, H, W) tensor, got "
+                              f"{tuple(x.shape)}")
+    B, _, H, W = x.shape
+    if tuple(out.shape) != (B, H, W, 3) or not out.is_contiguous():
+        raise _lib.IdiffError(f"decode_to_image: out must be a contiguous {(B, H, W, 3)} tensor, got "
+                              f"{tuple(out.shape)}")
+    if out.device != x.device:
+        raise _lib.IdiffError(f"decode_to_image: x on {x.device}, out on {out.device}")
+    check(_launch("decode_to_image", 0.0, (x.element_size() + 1.0) * x.numel(), lambda: lib.idiff_decode_to_image(
+        x.data_ptr(), int(x.dtype == torch.float32), out.data_ptr(), B, H * W, _stream())), "idiff_decode_to_image")
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # CLIP text encoder pieces (csrc/clip.cu)
 # ------------------------------------------------------------------------------------------------
