@@ -62,6 +62,12 @@ struct AttnCfg {
   static constexpr int SMEM_BYTES = 1024 + Q_BYTES + STAGES * 2 * KV_TILE_BYTES + 256;  // + alignment slack, barriers
 };
 
+// P is stored as 2^(s*c - m*c + P_LOG2_BIAS) <= 2^15 before it is rounded to 16 bits: unbiased, fp16 P would go
+// subnormal (an absolute step of 2^-24) for keys more than 2^-14 below the row max, and the sum of those rounding errors
+// over thousands of keys can exceed the relative precision of the output.  With the bias fp16 P stays normal down to
+// 2^-29 of the max.  The bias scales O and l alike and cancels in O / l; alpha is a difference of maxima and unaffected.
+constexpr float P_LOG2_BIAS = 15.f;
+
 template <int D, bool MASKED>
 __global__ void __launch_bounds__(AttnCfg<D>::THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK0,
@@ -201,7 +207,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       wgmma_commit();
     };
     // online softmax of the scores of key block j (rows rl0, rl0 + 8; a row's BKV scores are spread over
-    // the quad): sc becomes P = 2^(s*c - m*c) in place, alpha the factor O has to be rescaled by
+    // the quad): sc becomes P = 2^(s*c - m*c + P_LOG2_BIAS) in place, alpha the factor O has to be rescaled by
     auto softmax = [&](int j) {
       const bool seg1 = j >= T0;
       const int key0 = seg1 ? (j - T0) * BKV : j * BKV;  // first key of the block within its segment
@@ -259,7 +265,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
         alpha[hh] = exp2_approx((m_run[hh] - m_use) * c);  // m_run = -inf -> 0
         m_run[hh] = m_new;
-        mc[hh] = m_use * c;
+        mc[hh] = fmaf(m_use, c, -P_LOG2_BIAS);
         l_part[hh] *= alpha[hh];
       }
 #pragma unroll

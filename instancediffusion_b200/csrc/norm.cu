@@ -5,6 +5,13 @@
 // are bit-reproducible and independent of how many samples share a launch.  SiLU
 // (openaimodel.py:184,208,462) is fused into the GroupNorm apply pass.
 //
+// GroupNorm statistics are one-pass sums taken about a per-(sample, group) shift K, the group's first
+// element at pixel 0 of the sample: S = sum(x - K), Q = sum((x - K)^2), mean = K + S/n,
+// var = max(Q/n - (S/n)^2, 0).  Unshifted, E[x^2] - E[x]^2 cancels like (mean/std)^2 in fp32 (rstd off by
+// ~1e-3 at mean = 100 std, and the variance of a constant group is not 0); with the shift the cancellation
+// is relative to |mean - K| = O(std).  K depends only on the sample's own data, so batch invariance holds.
+// The output is (x - mean) * rstd * gamma + beta, so a constant group maps to exactly beta.
+//
 // Thread mapping (both GroupNorm passes): a CTA has k * CV threads, CV = C/8 16-byte vectors per
 // pixel; thread (r, cv) owns vector cv of pixels r, r+k, ... of the CTA's pixel chunk, so every
 // warp-wide request is a run of consecutive 16-byte vectors and each thread keeps several
@@ -17,6 +24,22 @@ namespace idiff {
 
 constexpr int GN_MAX_GROUPS = 32;
 constexpr int GN_MAX_CHUNKS = 64;  // pixel chunks per sample (two per lane in the apply pass's statistics reduction)
+
+// GroupNorm shift of the group starting at channel c0: its first element at pixel 0 (xs: the sample's pixel 0)
+IDIFF_DEVICE float gn_shift(const uint4* xs, int c0) { return h2f(reinterpret_cast<const h16*>(xs)[c0]); }
+// ... of each of the 8 channels c, c + 1, ... of a 16-byte vector (one division, not eight)
+IDIFF_DEVICE void gn_shift8(const uint4* xs, int c, int cpg, float (&sh)[8]) {
+  int c0 = (c / cpg) * cpg;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    while (c + j >= c0 + cpg) c0 += cpg;
+    sh[j] = gn_shift(xs, c0);
+  }
+}
+
+// SiLU of the apply passes: x / (1 + e^-x) as __fdividef (approximate reciprocal and a multiply, <= 2 ulp) instead of an
+// IEEE division, which pays for the subtraction of the mean; a denominator above 2^126 (x < -87) gives -0.
+IDIFF_DEVICE float gn_silu(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 
 IDIFF_DEVICE void unpack8(const uint4& v, float (&f)[8]) {
   const uint32_t u[4] = {v.x, v.y, v.z, v.w};
@@ -42,8 +65,10 @@ gn_stats_kernel(const uint4* __restrict__ x, float* __restrict__ partial, int hw
   const int b = blockIdx.y;
   const int p0 = blockIdx.x * pix_per_block;
   const int p1 = min(hw, p0 + pix_per_block);
+  const int cpg = C / groups;
   const uint4* xb = x + (long)b * hw * CV + cv;
-  float s[8], ss[8];
+  float s[8], ss[8], sh[8];
+  gn_shift8(x + (long)b * hw * CV, cv * 8, cpg, sh);
 #pragma unroll
   for (int j = 0; j < 8; ++j) s[j] = ss[j] = 0.f;
   int pix = p0 + r;
@@ -57,8 +82,9 @@ gn_stats_kernel(const uint4* __restrict__ x, float* __restrict__ partial, int hw
       unpack8(v[u], f);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        s[j] += f[j];
-        ss[j] += f[j] * f[j];
+        const float d = f[j] - sh[j];
+        s[j] += d;
+        ss[j] += d * d;
       }
     }
   }
@@ -67,8 +93,9 @@ gn_stats_kernel(const uint4* __restrict__ x, float* __restrict__ partial, int hw
     unpack8(xb[(long)pix * CV], f);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      s[j] += f[j];
-      ss[j] += f[j] * f[j];
+      const float d = f[j] - sh[j];
+      s[j] += d;
+      ss[j] += d * d;
     }
   }
 #pragma unroll
@@ -81,7 +108,6 @@ gn_stats_kernel(const uint4* __restrict__ x, float* __restrict__ partial, int hw
   // multiple of 32 (e.g. 240 for C=320): the trailing partial warp must not take part -- it would
   // shuffle with absent lanes and write the same `partial` slots as a full warp.
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nfull = blockDim.x >> 5;
-  const int cpg = C / groups;
   if (nfull == 0) {  // fewer than 32 threads (tiny maps through the C ABI): serial, still fixed order
     if (threadIdx.x == 0) {
       for (int g = 0; g < groups; ++g) {
@@ -119,7 +145,7 @@ gn_stats_kernel(const uint4* __restrict__ x, float* __restrict__ partial, int hw
   }
 }
 
-// grid (chunks, B), block k*CV
+// grid (chunks, B), block k*CV.  partial holds the shifted sums (S, Q) of gn_stats_kernel.
 __global__ void __launch_bounds__(512)
 gn_apply_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float* __restrict__ gamma,
                 const float* __restrict__ beta, const float* __restrict__ partial, int hw, int C,
@@ -138,18 +164,20 @@ gn_apply_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float*
     if (nfull == 0) {  // fewer than 32 threads (tiny maps through the C ABI): serial, same order
       if (threadIdx.x == 0)
         for (int g = 0; g < groups; ++g) {
+          const float kg = gn_shift(x + (long)b * hw * CV, g * cpg);
           float a = 0.f, q = 0.f;
           for (int ch = 0; ch < stat_chunks; ++ch) {
             const float2 v = *reinterpret_cast<const float2*>(partial + (((long)b * groups + g) * GN_MAX_CHUNKS + ch) * 2);
             a += v.x;
             q += v.y;
           }
-          const float mean = a * inv_n;
-          s_mean[g] = mean;
-          s_rstd[g] = rsqrtf(fmaxf(q * inv_n - mean * mean, 0.f) + eps);
+          const float dm = a * inv_n;  // mean - K
+          s_mean[g] = kg + dm;
+          s_rstd[g] = rsqrtf(fmaxf(q * inv_n - dm * dm, 0.f) + eps);
         }
     } else if (warp < nfull) {
       for (int g = warp; g < groups; g += nfull) {
+        const float kg = gn_shift(x + (long)b * hw * CV, g * cpg);  // issued with the partial loads, not after them
         float2 v = make_float2(0.f, 0.f);
         if (lane < stat_chunks) v = *reinterpret_cast<const float2*>(partial + (((long)b * groups + g) * GN_MAX_CHUNKS + lane) * 2);
         if (lane + 32 < stat_chunks) {
@@ -163,9 +191,9 @@ gn_apply_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float*
           v.y += __shfl_xor_sync(0xffffffffu, v.y, o);
         }
         if (lane == 0) {
-          const float mean = v.x * inv_n;
-          s_mean[g] = mean;
-          s_rstd[g] = rsqrtf(fmaxf(v.y * inv_n - mean * mean, 0.f) + eps);
+          const float dm = v.x * inv_n;  // mean - K
+          s_mean[g] = kg + dm;
+          s_rstd[g] = rsqrtf(fmaxf(v.y * inv_n - dm * dm, 0.f) + eps);
         }
       }
     }
@@ -173,14 +201,14 @@ gn_apply_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float*
   __syncthreads();
   const int r = threadIdx.x / CV;
   const int cv = threadIdx.x - r * CV;
-  float sa[8], sb[8];
+  float sm[8], sa[8], sb[8];  // y = (x - mean) * (rstd * gamma) + beta
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int c = cv * 8 + j;
     const int g = c / cpg;
-    const float a = s_rstd[g] * gamma[c];
-    sa[j] = a;
-    sb[j] = beta[c] - s_mean[g] * a;
+    sm[j] = s_mean[g];
+    sa[j] = s_rstd[g] * gamma[c];
+    sb[j] = beta[c];
   }
   const int p0 = blockIdx.x * pix_per_block;
   const int p1 = min(hw, p0 + pix_per_block);
@@ -191,11 +219,11 @@ gn_apply_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float*
     uint32_t o[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      float r0 = f[2 * j] * sa[2 * j] + sb[2 * j];
-      float r1 = f[2 * j + 1] * sa[2 * j + 1] + sb[2 * j + 1];
+      float r0 = (f[2 * j] - sm[2 * j]) * sa[2 * j] + sb[2 * j];
+      float r1 = (f[2 * j + 1] - sm[2 * j + 1]) * sa[2 * j + 1] + sb[2 * j + 1];
       if (fuse_silu) {
-        r0 = silu_f(r0);
-        r1 = silu_f(r1);
+        r0 = gn_silu(r0);
+        r1 = gn_silu(r1);
       }
       o[j] = pack_half2(r0, r1);
     }
@@ -259,9 +287,12 @@ gn_fused_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float*
   const int r = threadIdx.x / CV;
   const int cv = threadIdx.x - r * CV;
   const uint4* xb = x + ((long)b * hw + (long)rank * rows) * CVT + slab * CV + cv;
-  float s[8], ss[8];
+  float s[8], ss[8], sh[8];  // sums about the group shift (same K in every CTA of the cluster: pixel 0)
+  gn_shift8(x + (long)b * hw * CVT, slab * CS + cv * 8, cpg, sh);
 #pragma unroll
   for (int j = 0; j < 8; ++j) s[j] = ss[j] = 0.f;
+  // the shift of the slab group this thread turns into statistics after the exchange, loaded now, off that path
+  const float kg = threadIdx.x < ng ? gn_shift(x + (long)b * hw * CVT, slab * CS + threadIdx.x * cpg) : 0.f;
   int pix = r;
   for (; pix + 3 * k < rows; pix += 4 * k) {
     uint4 v[4];
@@ -274,8 +305,9 @@ gn_fused_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float*
       unpack8(v[u], f);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        s[j] += f[j];
-        ss[j] += f[j] * f[j];
+        const float d = f[j] - sh[j];
+        s[j] += d;
+        ss[j] += d * d;
       }
     }
   }
@@ -286,8 +318,9 @@ gn_fused_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float*
     unpack8(v, f);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      s[j] += f[j];
-      ss[j] += f[j] * f[j];
+      const float d = f[j] - sh[j];
+      s[j] += d;
+      ss[j] += d * d;
     }
   }
 #pragma unroll
@@ -324,20 +357,20 @@ gn_fused_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float*
       q += ld_dsmem_f32(&cta_part[threadIdx.x * 2 + 1], rk);
     }
     const float inv_n = 1.0f / (float)((long)cpg * hw);
-    const float mean = a * inv_n;
-    const float var = fmaxf(q * inv_n - mean * mean, 0.f);
-    s_mean[threadIdx.x] = mean;
+    const float dm = a * inv_n;  // mean - K
+    const float var = fmaxf(q * inv_n - dm * dm, 0.f);
+    s_mean[threadIdx.x] = kg + dm;
     s_rstd[threadIdx.x] = rsqrtf(var + eps);
   }
   cluster_sync_all();  // (also a CTA barrier) no CTA leaves while its partials may still be read
-  float sa[8], sb[8];
+  float sm[8], sa[8], sb[8];  // y = (x - mean) * (rstd * gamma) + beta
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int cl = cv * 8 + j;          // channel within the slab
     const int c = slab * CS + cl;       // channel of the tensor
-    const float a = s_rstd[cl / cpg] * gamma[c];
-    sa[j] = a;
-    sb[j] = beta[c] - s_mean[cl / cpg] * a;
+    sm[j] = s_mean[cl / cpg];
+    sa[j] = s_rstd[cl / cpg] * gamma[c];
+    sb[j] = beta[c];
   }
   uint4* yb = y + ((long)b * hw + (long)rank * rows) * CVT + slab * CV + cv;
   for (pix = r; pix < rows; pix += k) {
@@ -346,11 +379,11 @@ gn_fused_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const float*
     uint32_t o[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      float r0 = f[2 * j] * sa[2 * j] + sb[2 * j];
-      float r1 = f[2 * j + 1] * sa[2 * j + 1] + sb[2 * j + 1];
+      float r0 = (f[2 * j] - sm[2 * j]) * sa[2 * j] + sb[2 * j];
+      float r1 = (f[2 * j + 1] - sm[2 * j + 1]) * sa[2 * j + 1] + sb[2 * j + 1];
       if (fuse_silu) {
-        r0 = silu_f(r0);
-        r1 = silu_f(r1);
+        r0 = gn_silu(r0);
+        r1 = gn_silu(r1);
       }
       o[j] = pack_half2(r0, r1);
     }
@@ -397,7 +430,7 @@ layernorm40_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, const flo
   for (int j = 0; j < 40; ++j) s += v[j];
 #pragma unroll
   for (int o = LPR / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  const float mean = s * (1.0f / C);
+  const float mean = s / C;  // divided, not multiplied by a rounded 1/C: a constant row gets its exact value
   float ss = 0.f;
 #pragma unroll
   for (int j = 0; j < 40; ++j) {

@@ -165,7 +165,14 @@ def _req(t: torch.Tensor, dtype, name: str) -> None:
 
 class RowStats:
     """Per-row partial (sum, sum of squares) of a token matrix, fp32 [slots, rows, 2]: what a producer GEMM's
-    epilogue (or row_stats) leaves for the folded LayerNorm of the next GEMM (idiff_gemm_args.ln_*)."""
+    epilogue (or row_stats) leaves for the folded LayerNorm of the next GEMM (idiff_gemm_args.ln_*).
+
+    The consumer forms var = E[x^2] - E[x]^2 from these sums, which cancels like (mean/std)^2 in fp32, so the fold is
+    accurate for rows whose mean is within about 30 standard deviations of 0 (tests/test_conditioning_gpu.py asserts
+    r = mean/std <= 30 against float64).  Measured beyond that on an H100, C in {320, 640, 1280}, largest error over
+    max |output| of the plain and GEGLU consumers: r = 100: 2.7e-3 (fp16 build) / 2.6e-2 (bf16 build) from producer
+    statistics, 1.3e-3 / 3.2e-3 from row_stats; r = 300: 1.6e-2 / 0.23 from producer statistics, 1.5e-2 / 5.5e-3
+    from row_stats."""
     __slots__ = ("t", "slots")
 
     def __init__(self, t: torch.Tensor, slots: int):
@@ -184,7 +191,8 @@ class LnFold:
 def fold_layernorm(weight: torch.Tensor, bias: Optional[torch.Tensor], ln_weight: torch.Tensor, ln_bias: torch.Tensor,
                    eps: float, pack=None) -> LnFold:
     """LN(x) W^T + b = rstd (x W'^T - mean colsum(W')) + (W beta + b), W' = W * gamma (fp32 masters in).
-    `pack(w16, b32) -> (w16, b32)` re-lays rows out (GEGLU interleave) before the column sums are taken."""
+    `pack(w16, b32) -> (w16, b32)` re-lays rows out (GEGLU interleave) before the column sums are taken.
+    Range: rows with |mean| up to about 30 standard deviations (see RowStats for the measured errors beyond)."""
     W = weight.detach().float()
     g = ln_weight.detach().float()
     beta = ln_bias.detach().float()
