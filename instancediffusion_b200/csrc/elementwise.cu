@@ -260,9 +260,10 @@ __global__ void latent_mean_kernel(const float* const* __restrict__ xs, int coun
 // input conv of the UNet (openaimodel.py:469-480) with the conv chosen per image: 3x3, padding 1,
 // 4 -> cout channels.  One CTA per CONV_IN_ROWS output rows of one image, one thread per channel
 // pair: the thread keeps its 2 x 36 weights in registers and walks the rows, reading the 3x3x4
-// neighbourhood of each pixel from a shared tile of storage-rounded inputs.
+// neighbourhood of each pixel from a shared tile of storage-rounded inputs.  One row per CTA: a
+// 2-image 64x64 forward then launches 128 CTAs, enough to spread over the SMs.
 // ---------------------------------------------------------------------------------------------
-constexpr int CONV_IN_ROWS = 4;
+constexpr int CONV_IN_ROWS = 1;
 
 __global__ void __launch_bounds__(512)
 conv_in_select_kernel(const float* __restrict__ x, const h16* __restrict__ w0, const float* __restrict__ b0,

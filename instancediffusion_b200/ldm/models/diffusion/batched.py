@@ -327,12 +327,12 @@ class _RequestState:
 
     @staticmethod
     def evaluate(model, states: Sequence[_RequestState], forwards: Sequence[Tuple[List[Tuple[int, int]], Optional[int]]],
-                 scales: Sequence[float], flags: Sequence[bool], per_image_conv: bool = False):
+                 scales: Sequence[float], flags: Sequence[bool]):
         """One UNet evaluation of the trajectories of `forwards`, one forward per (chunk of (request, trajectory) slots,
         padded size), each request's images at its fuser scale and conv flag: {(request, trajectory): (e_c, e_u|None)}.
         A chunk with a padded size is filled up to it with copies of its last input (same context and grounding, so
         its hoisted tensors come from the caches) with a zero latent, fuser scale 0 and the model's own conv; their
-        outputs are dropped.  per_image_conv: see UNetModel.forward_batched."""
+        outputs are dropped."""
         out = {}
         for chunk, padded in forwards:
             inputs, sc, rs = [], [], []
@@ -353,7 +353,7 @@ class _RequestState:
                 inputs += [pad] * n_pad
                 sc += [0.0] * n_pad
                 rs += [False] * n_pad
-            outs = model.forward_batched(inputs, scales=sc, restored=rs, per_image_conv=per_image_conv)
+            outs = model.forward_batched(inputs, scales=sc, restored=rs)
             j = 0
             for r, k in chunk:
                 if states[r].plan.cfg:

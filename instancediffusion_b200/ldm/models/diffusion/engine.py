@@ -26,7 +26,7 @@ length, and of any strength, share forwards.  The engine adds admission, the gro
 The evaluations of a tick are grouped by (latent H x W, context length) in admission order, split into forwards of
 at most `max_batch` images by `plan_chunks`, and each forward is padded to the smallest of `buckets` that holds it.
 The forwards choose the fuser scale and the input conv per image on the device (`UNetModel.forward_batched(scales=,
-per_image_conv=True)`), so the captured CUDA graphs do not depend on the composition of the batch: per latent size,
+restored=)`), so the captured CUDA graphs do not depend on the composition of the batch: per latent size,
 context length, mask presence and fuser state (off / per image / one common scale) there are at most len(buckets).
 The engine never calls set_alpha_scale or swaps the model's first conv.
 
@@ -184,7 +184,7 @@ class SamplingEngine:
         n_graphs = len(model._graphs)
         with _RequestState.cache_bounds(model, sum(st.plan.trajectories + 1 for st in states) + 8,
                                         len(model._cat_cache) + len(forwards) + 1, self._pool):
-            evals = _RequestState.evaluate(model, states, forwards, scales, flags, per_image_conv=True)
+            evals = _RequestState.evaluate(model, states, forwards, scales, flags)
         self.graphs_captured += len(model._graphs) - n_graphs
         model.trim_concats(len(forwards))
         self.forwards += len(forwards)

@@ -73,31 +73,20 @@ class TimestepEmbedSequential(nn.Sequential, TimestepBlock):
             elif isinstance(layer, SpatialTransformer):
                 x = layer(x, context, objs, grounding_input, drop_box_mask=drop_box_mask)
             elif isinstance(layer, nn.Conv2d):
-                x = _conv3x3_module_forward(layer, x)
+                x = _conv_in_module_forward(layer, x)
             else:
                 x = layer(x)
         return x
 
 
-def _conv3x3_module_forward(conv: nn.Conv2d, x: torch.Tensor) -> torch.Tensor:
-    """nn.Conv2d(4, 320, 3, padding=1) holder of input_blocks[0] run through the conv kernel."""
-    x16, B, H, W = nchw_to_nhwc16(x)
-    cin = x16.shape[-1]
-    cpad = (cin + 63) // 64 * 64
-    if cpad != cin:
-        xp = torch.zeros((x16.shape[0], cpad), dtype=half(), device=x16.device)
-        xp[:, :cin] = x16
-        x16 = xp
-    wp = _pack_conv3x3_padded(conv.weight, cpad)
-    y = ops.gemm(x16, wp, f32(conv.bias), conv=(B, H, W, cpad))
+def _conv_in_module_forward(conv: nn.Conv2d, x: torch.Tensor) -> torch.Tensor:
+    """nn.Conv2d(4, 320, 3, padding=1) holder of input_blocks[0] run through the input conv kernel: the conv's own
+    taps as both weight sets, every image on the first."""
+    B, _, H, W = x.shape
+    w, b = pack_conv3x3_taps(w16(conv.weight)), f32(conv.bias)
+    flags = torch.zeros(B, dtype=torch.int32, device=x.device)
+    y = ops.conv_in_select(x.float(), w, b, w, b, flags)
     return nhwc16_to_nchw(y, B, H, W, x.dtype)
-
-
-def _pack_conv3x3_padded(weight: torch.Tensor, cin_pad: int) -> torch.Tensor:
-    cout, cin = weight.shape[:2]
-    w = torch.zeros((cout, cin_pad, 3, 3), dtype=half(), device=weight.device)
-    w[:, :cin] = weight.detach().to(half())
-    return pack_conv3x3(w)
 
 
 class Upsample(PackedModule):
@@ -324,7 +313,8 @@ class UNetModel(PackedModule):
         self._obj_cache: Dict = {}
         self._cat_cache: Dict = {}
         self._graphs: Dict = {}
-        self._in_packs: Dict = {}
+        self._in_convs = None
+        self._sd_conv_src = None
         self.use_cuda_graph = os.environ.get("IDIFF_CUDA_GRAPH", "1") != "0"
 
     # ------------------------------------------------------------------------------------------
@@ -358,66 +348,63 @@ class UNetModel(PackedModule):
     def set_sd_first_conv(self, sd_weights: Dict[str, torch.Tensor]):
         conv = self.input_blocks[0][0]
         device = conv.weight.device
-        self.first_conv_state_dict = deepcopy(conv.state_dict())
+        if not getattr(self, "_first_conv_restored", False):  # (a second call keeps the model's own conv)
+            self.first_conv_state_dict = deepcopy(conv.state_dict())
         new = conv_nd(2, 4, 320, 3, padding=1)
         new.load_state_dict(sd_weights)
         self.input_blocks[0][0] = new.to(device)
         self._first_conv_restored = True
-        # The packed first-conv weights of both states are kept alive side by side (the captured CUDA
-        # graphs of either state point at them), so swapping costs nothing and invalidates nothing --
-        # unless different SD weights than last time are supplied.
-        if getattr(self, "_sd_conv_src", None) is not sd_weights:
-            self._sd_conv_src = sd_weights
-            self._in_packs.pop((True, False), None)
-            self._in_packs.pop((True, True), None)
-            for k in [k for k in self._graphs if k[-1]]:
-                del self._graphs[k]
+        self._sd_conv_src = sd_weights
+        if self._in_convs is not None:  # in place: the captured graphs read these buffers
+            self._write_sd_conv(self.input_blocks[0][0].state_dict())
 
     def undo_first_conv_restore(self):
         """Not in the reference (whose swap is permanent within a process): lets a long-lived server /
         the benchmark run several `sample()` calls on one model object."""
         if getattr(self, "_first_conv_restored", False):
-            conv = conv_nd(2, 4, 320, 3, padding=1)  # a new module: packs built from the SD conv keep their tensors
+            conv = conv_nd(2, 4, 320, 3, padding=1)
             conv.load_state_dict(self.first_conv_state_dict)
             self.input_blocks[0][0] = conv.to(self.input_blocks[0][0].weight.device)
             self._first_conv_restored = False
 
-    def _in_conv_pack(self, restored: Optional[bool] = None, taps: bool = False):
-        """Packed input conv of the model's current first-conv state, or (restored=True / False) of the SD1.5 /
-        the model's own conv whatever the current state is.  The SD weights are the ones last given to
-        set_sd_first_conv, else load_sd_first_conv().  taps: in the layout of ops.conv_in_select instead of the
-        conv GEMM's."""
-        cur = bool(getattr(self, "_first_conv_restored", False))
-        key = cur if restored is None else bool(restored)
-        hit = self._in_packs.get((key, taps))
-        if hit is None:
+    def _in_conv(self):
+        """(w_own, b_own, w_sd, b_sd) of ops.conv_in_select: the model's own input conv (first_conv_state_dict while the
+        SD1.5 conv is swapped in) and the SD1.5 one -- the weights last given to set_sd_first_conv, else
+        load_sd_first_conv(), looked up once.  Until the SD1.5 weights are known (`_sd_conv_known`) the second set holds
+        the model's own conv, and forward_batched lets no image select it.  Allocated once and kept until
+        _drop_derived, as the captured graphs point at them; set_sd_first_conv writes new SD1.5 weights in place."""
+        if self._in_convs is None:
             conv0 = self.input_blocks[0][0]
-            if key == cur:
-                w, b = conv0.weight, conv0.bias
-            else:
-                sd = self.first_conv_state_dict if cur else getattr(self, "_sd_conv_src", None)
-                if sd is None:
+            restored = getattr(self, "_first_conv_restored", False)
+            own = self.first_conv_state_dict if restored else conv0.state_dict()
+            sd = conv0.state_dict() if restored else self._sd_conv_src
+            if sd is None:
+                try:
                     sd = self.load_sd_first_conv()
-                w, b = sd["weight"].to(conv0.weight.device), sd["bias"].to(conv0.weight.device)
+                except FileNotFoundError:
+                    pass
+            dev = conv0.weight.device
             with torch.no_grad():
-                hit = (pack_conv3x3_taps(w.detach().to(half())) if taps else _pack_conv3x3_padded(w, 64), f32(b))
-            self._in_packs[(key, taps)] = hit
-        return hit
+                w = pack_conv3x3_taps(own["weight"].to(dev).detach().to(half()))
+                b = f32(own["bias"].to(dev))
+            self._in_convs = (w, b, w.clone(), b.clone())
+            self._sd_conv_known = False
+            if sd is not None:
+                self._write_sd_conv(sd)
+        return self._in_convs
 
-    def _in_conv_taps(self):
-        """((w0, b0, w1, b1) of ops.conv_in_select: the model's own input conv and the SD1.5 one, whether the SD1.5
-        weights exist).  Without them both sets are the model's own conv, and no image may select the second."""
-        own = self._in_conv_pack(False, taps=True)
-        try:
-            return own + self._in_conv_pack(True, taps=True), True
-        except FileNotFoundError:
-            return own + own, False
+    def _write_sd_conv(self, sd: Dict[str, torch.Tensor]):
+        w_sd, b_sd = self._in_convs[2:]
+        with torch.no_grad():
+            w_sd.copy_(pack_conv3x3_taps(sd["weight"].to(w_sd.device).detach().to(half())))
+            b_sd.copy_(sd["bias"].to(b_sd.device))
+        self._sd_conv_known = True
 
     def _drop_derived(self):
         """Everything computed from the weights: packed first conv, captured graphs, hoisted text K/V and
         object tokens / per-fuser K/V (including the null-branch entry)."""
-        if hasattr(self, "_in_packs"):
-            self._in_packs.clear()
+        if hasattr(self, "_graphs"):
+            self._in_convs = None
             self._graphs.clear()
             self._ctx_cache.clear()
             self._obj_cache.clear()
@@ -580,13 +567,12 @@ class UNetModel(PackedModule):
         return any(blk.fuser.scale != 0 for st in self._transformers() for blk in st.transformer_blocks)
 
     def _core(self, x: torch.Tensor, t: torch.Tensor, ctx_kv_all: torch.Tensor, M: int,
-              obj_kvs: Optional[List[torch.Tensor]], n_obj: int, mask=None, fuser_scale=None,
-              n_restored=None) -> torch.Tensor:
+              obj_kvs: Optional[List[torch.Tensor]], n_obj: int, mask, fuser_scale,
+              conv_flags: torch.Tensor) -> torch.Tensor:
         """x fp32 (B,4,H,W), t fp32 (B,), ctx_kv_all fp16 [B*M, sumKV], obj_kvs per-fuser [B*n_obj, 2C]
         (or None on alpha=0 steps) -> eps fp32 (B,4,H,W).  fuser_scale: None (each fuser's `.scale`), a float or
-        an fp32 [B] tensor of per-image scales.  n_restored: None (the model's first-conv state for every image),
-        the number of trailing images that take the SD1.5 input conv, the others the model's own, or an int32 [B]
-        device tensor of per-image flags (1: the SD1.5 conv) for ops.conv_in_select."""
+        an fp32 [B] tensor of per-image scales.  conv_flags: int32 [B] device tensor, per image the input conv of
+        ops.conv_in_select (0: the model's own, 1: the SD1.5 one)."""
         p = self.pk()
         B, _, H, W = x.shape
         # time embedding (openaimodel.py:497-498) ; SiLU of emb_layers[0] folded into the last epilogue
@@ -627,19 +613,7 @@ class UNetModel(PackedModule):
                     raise TypeError(f"unexpected layer {type(layer)}")
             return h, hh, ww
 
-        if isinstance(n_restored, torch.Tensor):
-            h = ops.conv_in_select(x, *self._in_conv_taps()[0], n_restored)
-        elif n_restored is None or n_restored in (0, B):
-            x16 = ops.nchw_f32_to_nhwc_f16(x, 64)
-            w_in, b_in = self._in_conv_pack(None if n_restored is None else n_restored == B)
-            h = ops.gemm(x16, w_in, b_in, conv=(B, H, W, 64))
-        else:  # one conv GEMM per first-conv state, each on its contiguous range of images
-            x16 = ops.nchw_f32_to_nhwc_f16(x, 64)
-            h = torch.empty((B * H * W, self.model_channels), dtype=half(), device=x.device)
-            for b0, nb, restored in ((0, B - n_restored, False), (B - n_restored, n_restored, True)):
-                w_in, b_in = self._in_conv_pack(restored)
-                rows = slice(b0 * H * W, (b0 + nb) * H * W)
-                ops.gemm(x16[rows], w_in, b_in, conv=(nb, H, W, 64), out=h[rows])
+        h = ops.conv_in_select(x, *self._in_conv(), conv_flags)
         hh, ww = H, W
         hs = [(h, hh, ww)]
         for module in list(self.input_blocks)[1:]:
@@ -734,19 +708,18 @@ class UNetModel(PackedModule):
 
     @torch.no_grad()
     def forward_batched(self, inputs: List[dict], *, scales: Optional[List[float]] = None,
-                        restored: Optional[List[bool]] = None, per_image_conv: bool = False) -> List[torch.Tensor]:
+                        restored: Optional[List[bool]] = None) -> List[torch.Tensor]:
         """Run several independent forwards as one batch; returns one eps tensor per input.
 
         scales: one fuser scale per input -- what set_alpha_scale would set for a forward of that input alone --
         instead of the fusers' own `.scale`.  Equal scales run the scalar-gate path (all 0: the fusers are skipped);
         mixed scales run the fusers on every image with the gates tanh(alpha) * scale of each image.  In batch-invariant
-        mode (ops.set_batch_invariant) any non-zero scale takes the per-image gates, and every input conv is per image
-        as with per_image_conv.
+        mode (ops.set_batch_invariant) any non-zero scale takes the per-image gates.
         restored: per input, True = the SD1.5 input conv that restore_first_conv_from_SD swaps in, False = the
         model's own; the model's conv is not swapped.  Default: the model's current first-conv state.
-        per_image_conv: choose each image's input conv on the device (ops.conv_in_select) from a per-image flag that,
-        like the per-image scales, is a static input of the captured graph.  The count of SD1.5-conv images then
-        stays out of the graph key, and the images keep their order."""
+        Each image's input conv is chosen on the device (ops.conv_in_select) from a per-image flag that, like the
+        per-image scales, is a static input of the captured graph, so the graphs do not depend on which images take
+        which conv."""
         # storage type or batch-invariant mode switched: derived tensors and captured graphs are stale
         if getattr(self, "_storage_epoch", None) != (ops.STORAGE_EPOCH, ops.MODE_EPOCH):
             self._drop_derived()
@@ -756,8 +729,8 @@ class UNetModel(PackedModule):
             if arg is not None and len(arg) != n:
                 raise ValueError(f"forward_batched: {len(arg)} {name} for {n} inputs")
         sizes = [inp["x"].shape[0] for inp in inputs]
-        # batch-invariant mode: one arithmetic path per image whatever the call -- every input conv runs per image
-        # (ops.conv_in_select), and fusers run with per-image gates unless every image skips them
+        # batch-invariant mode: one arithmetic path per image whatever the call -- fusers run with per-image gates
+        # unless every image skips them
         invariant = ops.batch_invariant()
         if invariant and scales is None:
             own = {float(blk.fuser.scale) for st in self._transformers() for blk in st.transformer_blocks}
@@ -765,43 +738,32 @@ class UNetModel(PackedModule):
                 raise ValueError(f"forward_batched: batch-invariant mode needs one fuser scale for the model, the "
                                  f"fusers have {sorted(own)}; pass scales= instead")
             scales = [own.pop()] * n
-        if per_image_conv or invariant:
-            order = list(range(n))
-            cur = bool(getattr(self, "_first_conv_restored", False))
-            flags = [bool(restored[i]) if restored is not None else cur for i in range(n)]
-            if any(flags):
-                self._in_conv_pack(True, taps=True)  # raises when no SD1.5 conv weights exist
-            rows_in = torch.tensor([int(f) for f, b in zip(flags, sizes) for _ in range(b)], dtype=torch.int32)
-            n_restored = rows_in.pin_memory().to(inputs[0]["x"].device, non_blocking=True)
-        elif restored is None:
-            order = list(range(n))
-            n_restored = sum(sizes) if getattr(self, "_first_conv_restored", False) else 0
-        else:  # images of the SD1.5 conv last: each input conv is one GEMM over a contiguous range of images
-            order = [i for i in range(n) if not restored[i]] + [i for i in range(n) if restored[i]]
-            n_restored = sum(sizes[i] for i in range(n) if restored[i])
-        ins = [inputs[i] for i in order]
         fuser_scale, active = None, None
         if scales is not None:
-            s = [float(scales[i]) for i in order]
+            s = [float(v) for v in scales]
             if all(v == s[0] for v in s) and not (invariant and s[0] != 0):
                 fuser_scale, active = s[0], s[0] != 0
             else:
-                rows = torch.tensor([v for v, i in zip(s, order) for _ in range(sizes[i])], dtype=torch.float32)
-                fuser_scale, active = rows.pin_memory().to(ins[0]["x"].device, non_blocking=True), True
-        x, t, ctx, M, okv, n_obj, mask = self._gather_inputs(ins, active)
-        eps = self._run_core(x, t, ctx, M, okv, n_obj, mask, fuser_scale, n_restored)
-        outs = torch.split(eps, [sizes[i] for i in order], 0)
-        res = [None] * n
-        for j, i in enumerate(order):
-            res[i] = outs[j]
-        return res
+                rows = torch.tensor([v for v, b in zip(s, sizes) for _ in range(b)], dtype=torch.float32)
+                fuser_scale, active = rows.pin_memory().to(inputs[0]["x"].device, non_blocking=True), True
+        x, t, ctx, M, okv, n_obj, mask = self._gather_inputs(inputs, active)
+        if restored is None:
+            restored = [getattr(self, "_first_conv_restored", False)] * n
+        self._in_conv()
+        if any(restored) and not self._sd_conv_known:
+            self._write_sd_conv(self.load_sd_first_conv())  # raises when no SD1.5 conv weights exist
+        flags = torch.tensor([int(bool(r)) for r, b in zip(restored, sizes) for _ in range(b)], dtype=torch.int32)
+        conv_flags = flags.pin_memory().to(x.device, non_blocking=True)
+        eps = self._run_core(x, t, ctx, M, okv, n_obj, mask, fuser_scale, conv_flags)
+        return list(torch.split(eps, sizes, 0))
 
-    def _run_core(self, x, t, ctx, M, okv, n_obj, mask=None, fuser_scale=None, n_restored=None):
+    def _run_core(self, x, t, ctx, M, okv, n_obj, mask, fuser_scale, conv_flags):
         if not self.use_cuda_graph:
-            return self._core(x, t, ctx, M, okv, n_obj, mask, fuser_scale, n_restored)
+            return self._core(x, t, ctx, M, okv, n_obj, mask, fuser_scale, conv_flags)
         # the fuser gates scale*tanh(alpha) are kernel arguments, frozen into a captured graph: the
         # per-fuser scales (set_alpha_scale may set any value, alpha_generator's decay stage is
-        # fractional) are part of the key.  Per-image scales are a static input buffer of the graph instead.
+        # fractional) are part of the key.  Per-image scales and conv flags are static input buffers of the graph
+        # instead, and it reads both input convs from the buffers of _in_conv.
         if okv is None:
             scales = ()
         elif isinstance(fuser_scale, torch.Tensor):
@@ -809,20 +771,12 @@ class UNetModel(PackedModule):
         else:
             scales = tuple(float(blk.fuser.scale if fuser_scale is None else fuser_scale)
                            for st in self._transformers() for blk in st.transformer_blocks)
-        if n_restored is None:
-            n_restored = x.shape[0] if getattr(self, "_first_conv_restored", False) else 0
-        # per-image conv flags are a static input buffer; the graph points at both packed convs (or twice at the
-        # model's own while no SD1.5 weights exist)
-        conv = n_restored
-        if isinstance(n_restored, torch.Tensor):
-            conv = "per-image" if self._in_conv_taps()[1] else "per-image, own conv only"
-        # (set_sd_first_conv drops the graphs whose last key entry, the count of SD-conv images, is truthy)
-        key = (tuple(x.shape), M, scales, n_obj, mask is not None, conv)
+        key = (tuple(x.shape), M, scales, n_obj, mask is not None)
         g = self._graphs.get(key)
         if g is None:
-            g = _CoreGraph(self, x, t, ctx, M, okv, n_obj, mask, fuser_scale, n_restored)
+            g = _CoreGraph(self, x, t, ctx, M, okv, n_obj, mask, fuser_scale, conv_flags)
             self._graphs[key] = g
-        return g.replay(x, t, ctx, okv, mask, fuser_scale, n_restored)
+        return g.replay(x, t, ctx, okv, mask, fuser_scale, conv_flags)
 
     def forward_single_input(self, input):
         return self.forward_batched([input])[0]
@@ -835,7 +789,7 @@ class _CoreGraph:
     """One captured CUDA graph of UNetModel._core for a fixed (batch, shapes, fuser on/off) key.
     Inputs are copied into static buffers, the graph is replayed, the static output is cloned."""
 
-    def __init__(self, model: UNetModel, x, t, ctx, M, okv, n_obj, mask=None, fuser_scale=None, n_restored=None):
+    def __init__(self, model: UNetModel, x, t, ctx, M, okv, n_obj, mask, fuser_scale, conv_flags):
         self.x = x.clone()
         self.t = t.clone()
         self.ctx = ctx.clone()
@@ -843,7 +797,7 @@ class _CoreGraph:
         self.mask = (mask[0].clone(), mask[1].clone()) if mask is not None else None
         # per-image fuser scales: a static input like x and t (a float or None is part of the graph key)
         self.scale = fuser_scale.clone() if isinstance(fuser_scale, torch.Tensor) else fuser_scale
-        self.conv = n_restored.clone() if isinstance(n_restored, torch.Tensor) else n_restored
+        self.conv = conv_flags.clone()
         model.pk()  # make sure packing (allocations + host work) happens outside capture
         for st in model._transformers():
             st.pk()
@@ -865,13 +819,12 @@ class _CoreGraph:
             with torch.cuda.graph(self.graph, pool=model.graph_pool):
                 self.out = model._core(self.x, self.t, self.ctx, M, self.okv, n_obj, self.mask, self.scale, self.conv)
 
-    def replay(self, x, t, ctx, okv, mask=None, fuser_scale=None, n_restored=None):
+    def replay(self, x, t, ctx, okv, mask, fuser_scale, conv_flags):
         self.x.copy_(x)
         self.t.copy_(t)
         if isinstance(self.scale, torch.Tensor):
             self.scale.copy_(fuser_scale)
-        if isinstance(self.conv, torch.Tensor):
-            self.conv.copy_(n_restored)
+        self.conv.copy_(conv_flags)
         # step-invariant inputs: the static buffers already hold them when the very same (immutable, cached)
         # tensor objects come back -- every step of a sampling run after the first
         last = getattr(self, "_last", (None, None, None))

@@ -45,7 +45,7 @@ class FakeUNet(torch.nn.Module):
     def restore_first_conv_from_SD(self):
         self._first_conv_restored = True
 
-    def forward_batched(self, inputs, *, scales=None, restored=None, per_image_conv=False):
+    def forward_batched(self, inputs, *, scales=None, restored=None):
         n = len(inputs)
         scales = [float(self.fusers[0].scale)] * n if scales is None else scales
         restored = [self._first_conv_restored] * n if restored is None else restored

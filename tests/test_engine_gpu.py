@@ -1,7 +1,6 @@
-"""`-m gpu` tests of continuous batching: the per-image input conv kernel (idiff_conv_in_select) against torch,
-UNetModel.forward_batched(per_image_conv=True) against separate forwards, and SamplingEngine with staggered arrivals
-against each request's own sampler run -- plus the graph bound, memory over repeated traces, two latent sizes at once
-and one request anchored to the reference's golden latent."""
+"""`-m gpu` tests of continuous batching: the per-image input conv kernel (idiff_conv_in_select) against torch, and
+SamplingEngine with staggered arrivals against each request's own sampler run -- plus the graph bound, memory over
+repeated traces, two latent sizes at once and one request anchored to the reference's golden latent."""
 import os
 import sys
 from functools import partial
@@ -65,50 +64,7 @@ def test_conv_in_select_matches_conv2d(cuda_device, dtype, B, H, W):
 
 
 # ------------------------------------------------------------------------------------------------
-# 2. forward_batched(per_image_conv=True)
-# ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("graph", [False, True])
-def test_forward_batched_per_image_conv(cuda_device, unet, graph):
-    from instancediffusion_b200 import synthetic
-    from instancediffusion_b200.utils.model import set_alpha_scale
-    gti = unet.grounding_tokenizer_input
-    ia, uca = synthetic.make_sampler_inputs(gti, 1, 2, 171, "box", device=cuda_device)
-    ib, _ = synthetic.make_sampler_inputs(gti, 1, 3, 172, "box", device=cuda_device)
-    ts = [torch.full((1,), t, dtype=torch.long, device=cuda_device) for t in (601, 801, 401, 201)]
-    inputs = [dict(x=ia["x"], timesteps=ts[0], context=ia["context"], grounding_input=ia["grounding_input"]),
-              dict(x=ia["x"], timesteps=ts[1], context=uca),
-              dict(x=ib["x"], timesteps=ts[2], context=ib["context"], grounding_input=ib["grounding_input"]),
-              dict(x=ib["x"] * 0.5, timesteps=ts[3], context=ib["context"], grounding_input=ib["grounding_input"])]
-    scales, restored = [1.0, 0.0, 0.5, 1.0], [True, False, True, False]
-    unet.use_cuda_graph = graph
-    try:
-        _reset(unet)
-        refs = []
-        for inp, s, r in zip(inputs, scales, restored):
-            set_alpha_scale(unet, s)
-            if r:
-                unet.restore_first_conv_from_SD()
-            refs.append(unet(dict(inp)).clone())
-            unet.undo_first_conv_restore()
-        set_alpha_scale(unet, 1)
-        for flags in (restored, [not r for r in restored]):  # a new flag pattern replays the same graph
-            n = len(unet._graphs)
-            got = unet.forward_batched(inputs, scales=scales, restored=flags, per_image_conv=True)
-            assert not unet._first_conv_restored
-            if flags is restored:
-                for k, (g, ref) in enumerate(zip(got, refs)):
-                    r = _rel(g, ref)
-                    print(f"[per_image_conv graph={graph}] input {k}: rel_l2 {r:.2e}")
-                    assert r < EPS_TOL, (k, r)
-            else:
-                assert len(unet._graphs) == n
-    finally:
-        _reset(unet)
-        unet.use_cuda_graph = True
-
-
-# ------------------------------------------------------------------------------------------------
-# 3. SamplingEngine
+# 2. SamplingEngine
 # ------------------------------------------------------------------------------------------------
 def _requests(unet, device):
     """Five requests: S in {10, 11, 20}; MIS 0.36 (one with the instance-isolation mask), MIS 1, plain PLMS, and one
@@ -146,16 +102,16 @@ def _drive(engine, reqs, ticks):
 
 def _graph_groups(keys):
     """Engine graph keys grouped by everything but the batch: (latent size, context length, fuser state, n_obj,
-    mask presence, conv) -> batch sizes."""
+    mask presence) -> batch sizes."""
     groups = {}
-    for shape, M, scales, n_obj, mask, conv in keys:
+    for shape, M, scales, n_obj, mask in keys:
         state = "off" if scales == () else ("per-image" if scales == ("per-image",) else "scalar")
-        groups.setdefault((shape[1:], M, state, scales, n_obj, mask, conv), set()).add(shape[0])
+        groups.setdefault((shape[1:], M, state, scales, n_obj, mask), set()).add(shape[0])
     return groups
 
 
 @pytest.mark.parametrize("graph", [False, True])
-def test_engine_staggered_requests_match_their_own_samplers(cuda_device, unet, diffusion, graph):
+def test_engine_staggered_arrivals_match_their_own_samplers(cuda_device, unet, diffusion, graph):
     from instancediffusion_b200.ldm.models.diffusion.engine import SamplingEngine
     reqs = _requests(unet, cuda_device)
     alone = [_run_alone(unet, diffusion, r, r.S) for r in reqs]

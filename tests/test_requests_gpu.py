@@ -127,12 +127,18 @@ def test_forward_batched_per_input_scale_and_first_conv(cuda_device, unet, graph
             refs.append(unet(dict(inp)).clone())
             unet.undo_first_conv_restore()
         set_alpha_scale(unet, 1)
-        got = unet.forward_batched(inputs, scales=scales, restored=restored)
-        assert not unet._first_conv_restored, "forward_batched(restored=...) must not swap the model's conv"
-        for k, (g, ref) in enumerate(zip(got, refs)):
-            r = _rel(g, ref)
-            print(f"[forward_batched graph={graph}] input {k} scale {scales[k]} restored {restored[k]}: rel_l2 {r:.2e}")
-            assert r < EPS_TOL, (k, r)
+        for flags in (restored, [not r for r in restored]):  # a new flag pattern replays the same graph
+            n = len(unet._graphs)
+            got = unet.forward_batched(inputs, scales=scales, restored=flags)
+            assert not unet._first_conv_restored, "forward_batched(restored=...) must not swap the model's conv"
+            if flags is restored:
+                for k, (g, ref) in enumerate(zip(got, refs)):
+                    r = _rel(g, ref)
+                    print(f"[forward_batched graph={graph}] input {k} scale {scales[k]} restored {restored[k]}: "
+                          f"rel_l2 {r:.2e}")
+                    assert r < EPS_TOL, (k, r)
+            else:
+                assert len(unet._graphs) == n
         # equal scales take the scalar path: the fusers' own scale does not matter
         set_alpha_scale(unet, 0)
         same = unet.forward_batched(inputs[:1] + inputs[2:3], scales=[1.0, 1.0])
@@ -140,6 +146,51 @@ def test_forward_batched_per_input_scale_and_first_conv(cuda_device, unet, graph
     finally:
         _reset(unet)
         unet.use_cuda_graph = True
+
+
+def test_sd_conv_given_after_capture_reaches_the_graph(cuda_device, monkeypatch):
+    """A graph captured before the SD1.5 conv weights are known is replayed after set_sd_first_conv gives them, and
+    again after it gives different ones: each replay runs the weights given last, as the eager forward does, and the
+    model's own conv for the other images."""
+    from instancediffusion_b200 import synthetic
+    from instancediffusion_b200.weights import build_unet
+    monkeypatch.delenv("IDIFF_PRETRAINED_DIR", raising=False)
+    model = build_unet("box", cuda_device, seed=0)
+    ia, uca = synthetic.make_sampler_inputs(model.grounding_tokenizer_input, 1, 2, 73, "box", device=cuda_device)
+    t = torch.full((1,), 501, dtype=torch.long, device=cuda_device)
+    inputs = [dict(x=ia["x"], timesteps=t, context=ia["context"], grounding_input=ia["grounding_input"]),
+              dict(x=ia["x"] * 0.5, timesteps=t, context=uca)]
+    scales, restored = [1.0, 0.5], [True, False]
+
+    def both():
+        model.use_cuda_graph = False
+        eager = model.forward_batched(inputs, scales=scales, restored=restored)
+        model.use_cuda_graph = True
+        return eager, model.forward_batched(inputs, scales=scales, restored=restored)
+
+    before = model.forward_batched(inputs, scales=scales)  # captured while no SD1.5 weights are known
+    n = len(model._graphs)
+    with pytest.raises(FileNotFoundError):
+        model.forward_batched(inputs, scales=scales, restored=restored)
+    sd_a = torch.load(os.path.join(GOLDEN, "sd15_first_conv.pt"), map_location="cpu")
+    g = torch.Generator().manual_seed(7)
+    sd_b = {k: v + 0.05 * torch.randn(v.shape, generator=g) for k, v in sd_a.items()}
+    got = []
+    for sd in (sd_a, sd_b):
+        model.set_sd_first_conv(sd)  # (the second call while the first SD1.5 conv is swapped in)
+        eager, graphed = both()
+        assert len(model._graphs) == n
+        for e, r in zip(eager, graphed):
+            assert torch.equal(e, r)
+        assert torch.equal(graphed[1], before[1])  # the model's own conv
+        got.append(graphed)
+    assert not torch.equal(got[0][0], got[1][0])
+    # packs built afresh from the model's state give what the in-place writes gave
+    model.invalidate_pack()
+    for e, r in zip(both()[0], got[1]):
+        assert torch.equal(e, r)
+    model.undo_first_conv_restore()
+    assert torch.equal(model.forward_batched(inputs, scales=scales)[1], before[1])
 
 
 # ------------------------------------------------------------------------------------------------

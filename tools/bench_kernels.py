@@ -3,7 +3,7 @@ images at 512^2).  Each shape: 3 warm-ups, then N timed launches bracketed by CU
 launching stream with an L2 flush (256 MB write) between launches.  Prints one table row per shape
 and a JSON blob (gpurun_out/kernels_<tag>.json).
 
-  python tools/bench_kernels.py [tag] [gemm|attn|norm|all] [--batch N] [--batch-invariant]
+  python tools/bench_kernels.py [tag] [gemm|attn|norm|conv_in|all] [--batch N] [--batch-invariant]
 
 --batch-invariant runs every kernel in batch-invariant mode (ops.set_batch_invariant), so per-shape costs of the
 two modes can be compared; --batch sets the forward batch (default 8).
@@ -17,7 +17,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from instancediffusion_b200 import ops  # noqa: E402
-from instancediffusion_b200.packing import pack_geglu  # noqa: E402
+from instancediffusion_b200.packing import pack_conv3x3, pack_conv3x3_taps, pack_geglu  # noqa: E402
 
 dev = torch.device("cuda:0")
 argv = [a for a in sys.argv[1:] if a != "--batch-invariant"]
@@ -216,6 +216,33 @@ if which in ("all", "norm"):
         by = 4.0 * (h.numel() + sk.numel())
         rows.append(dict(kind="scaleu", label=f"scaleu {hw} {c1}+{c2}", us=t * 1e6, gbs=by / t / 1e9))
         print(f"{f'scaleu {hw} {c1}+{c2}':30s} {t * 1e6:8.1f} {by / t / 1e9:14.0f}")
+
+if which in ("all", "conv_in"):
+    # The UNet input conv (4 -> 320, 3x3) as the model runs it, ops.conv_in_select, against the conv GEMM over a
+    # 64-channel zero-padded NHWC copy of the latent that the model ran before.  Batches: one request (2), config 2
+    # (8), a full engine bucket (32), a config 5 Multi-instance group (256) at 64x64, and config 4 (16 at 96x96, bf16).
+    print(f"\n{'input conv':30s} {'select us':>10s} {'gemm us':>10s} {'rel_l2':>8s}")
+    for nb, hw, dtype in ((2, 64, torch.float16), (8, 64, torch.float16), (32, 64, torch.float16),
+                          (256, 64, torch.float16), (16, 96, torch.bfloat16)):
+        with ops.storage(dtype):
+            x = torch.randn(nb, 4, hw, hw, device=dev)
+            w = torch.randn(320, 4, 3, 3, device=dev) * 0.2
+            bias = torch.randn(320, device=dev) * 0.1
+            wt = pack_conv3x3_taps(w.to(dtype))
+            flags = torch.zeros(nb, dtype=torch.int32, device=dev)
+            wpad = torch.zeros(320, 64, 3, 3, dtype=dtype, device=dev)
+            wpad[:, :4] = w.to(dtype)
+            wg = pack_conv3x3(wpad)
+            x16 = torch.empty((nb * hw * hw, 64), dtype=dtype, device=dev)
+            out = torch.empty((nb * hw * hw, 320), dtype=dtype, device=dev)
+            out_g = torch.empty_like(out)
+            sel = lambda: ops.conv_in_select(x, wt, bias, wt, bias, flags, out=out)
+            gem = lambda: ops.gemm(ops.nchw_f32_to_nhwc_f16(x, 64, out=x16), wg, bias, conv=(nb, hw, hw, 64), out=out_g)
+            ts, tg = timed(sel, iters=21), timed(gem, iters=21)
+            rel = ((out.float() - out_g.float()).norm() / out_g.float().norm()).item()
+        label = f"conv_in B{nb} {hw}x{hw} {str(dtype)[6:]}"
+        rows.append(dict(kind="conv_in", label=label, us=ts * 1e6, gemm_us=tg * 1e6, rel_l2=rel))
+        print(f"{label:30s} {ts * 1e6:10.1f} {tg * 1e6:10.1f} {rel:8.1e}")
 
 os.makedirs("gpurun_out", exist_ok=True)
 json.dump(rows, open(f"gpurun_out/kernels_{tag}.json", "w"), indent=1)

@@ -121,7 +121,7 @@ def main():
                     f"alpha 0.8 (requests {list(ALPHA_06)} at 0.6), fp16",
         "gpu": gpu_info(), "max_batch": args.max_batch, "reps": args.reps, "runs": runs,
         "speedup_best": best["sample_requests"] / best["sequential"],
-        "latent_rel_l2_vs_sequential": rel,
+        "latent_rel_l2_vs_sequential": rel, "graphs_captured": len(model._graphs),
     }
     print(json.dumps(line))
     if args.out:
