@@ -236,6 +236,20 @@ int idiff_ddim_update(const float* x, const float* e_c, const float* e_u, float 
                       float sigma, unsigned long long seed, int index, float* e_out, float* x_out, long n,
                       void* stream);
 /* ---------------------------------------------------------------------------------------------
+ * idiff_dpmpp2m_update: fused DPM-Solver++(2M) step (Lu et al. 2022, data prediction), all fp32, n elements:
+ *   e      = e_u + gs*(e_c - e_u)         (CFG; e_u may be NULL -> e = e_c)
+ *   x0     = (x - sigma_t*e) / alpha_t
+ *   D      = w_cur*x0 + w_prev*x0_prev    (x0_prev may be NULL -> D = w_cur*x0)
+ *   x_out  = c_x*x + c_d*D
+ * The host computes the scalars in float64 from alpha = sqrt(a), sigma = sqrt(1-a), lambda = log(alpha/sigma) and
+ * h = lambda_n - lambda_t: c_x = sigma_n/sigma_t, c_d = -alpha_n*expm1(-h); a first step has w_cur = 1 and no x0_prev,
+ * a later one w_cur = 1 + 1/(2r), w_prev = -1/(2r), r = h_prev/h.  x0_out (may be NULL) receives x0, the x0_prev of
+ * the next step.  alpha_t > 0.
+ * ------------------------------------------------------------------------------------------- */
+int idiff_dpmpp2m_update(const float* x, const float* e_c, const float* e_u, float gs, const float* x0_prev,
+                         float alpha_t, float sigma_t, float c_x, float c_d, float w_cur, float w_prev, float* x0_out,
+                         float* x_out, long n, void* stream);
+/* ---------------------------------------------------------------------------------------------
  * idiff_noise_latent: start latent of image-to-image sampling (SDEdit), all fp32, n elements:
  *   x_out[i] = sqrt_a*x_init[i % n_init] + sqrt_1m_a*z_i          (n % n_init == 0: x_init broadcast over the batch)
  * z_i is a standard normal that depends on (seed, i) alone: Philox4x32-10 with key (seed & 0xffffffff, seed >> 32)

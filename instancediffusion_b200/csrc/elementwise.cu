@@ -221,6 +221,32 @@ __global__ void ddim_update_kernel(const float* __restrict__ x, const float* __r
 }
 
 // ---------------------------------------------------------------------------------------------
+// fused DPM-Solver++(2M) update (Lu et al. 2022, Algorithm 2, data prediction)
+// ---------------------------------------------------------------------------------------------
+// The host folds the step's log-SNR quantities into fp32 scalars (c_x = sigma_n / sigma_t, c_d = -alpha_n expm1(-h),
+// the weights of D), so per element this is CFG, the x_0 prediction, the two-term D and one FMA pair.
+__global__ void dpmpp2m_update_kernel(const float* __restrict__ x, const float* __restrict__ e_c,
+                                      const float* __restrict__ e_u, float gs, const float* __restrict__ x0_prev,
+                                      float alpha_t, float sigma_t, float c_x, float c_d, float w_cur, float w_prev,
+                                      float* __restrict__ x0_out, float* __restrict__ x_out, long n) {
+  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
+  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    float e = e_c[i];
+    if (e_u) {
+      const float u = e_u[i];
+      e = u + gs * (e - u);
+    }
+    const float xi = x[i];
+    const float x0 = (xi - sigma_t * e) / alpha_t;
+    float d = w_cur * x0;
+    if (x0_prev) d += w_prev * x0_prev[i];
+    if (x0_out) x0_out[i] = x0;
+    x_out[i] = c_x * xi + c_d * d;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // image-to-image start latent: x_init noised to the start timestep (q_sample with a seeded z)
 // ---------------------------------------------------------------------------------------------
 // One thread per group of four elements 4c .. 4c+3: Philox4x32-10 at counter (c lo, c hi, 0, 1) and key (seed lo,
@@ -482,6 +508,17 @@ extern "C" int idiff_ddim_update(const float* x, const float* e_c, const float* 
   IDIFF_CHECK_CUDA(launch_pdl(ddim_update_kernel, dim3(grid_for(groups, 256)), dim3(256), 0,
                               reinterpret_cast<cudaStream_t>(stream), x, e_c, e_u, gs, sqrtf(a_t), sqrtf(1.0f - a_t),
                               sqrtf(a_prev), sqrt_dir, sigma, key, (uint32_t)index, e_out, x_out, n));
+  IDIFF_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int idiff_dpmpp2m_update(const float* x, const float* e_c, const float* e_u, float gs,
+                                    const float* x0_prev, float alpha_t, float sigma_t, float c_x, float c_d,
+                                    float w_cur, float w_prev, float* x0_out, float* x_out, long n, void* stream) {
+  IDIFF_REQUIRE(x && e_c && x_out && n > 0 && alpha_t > 0.f, "idiff_dpmpp2m_update: bad arguments");
+  IDIFF_CHECK_CUDA(launch_pdl(dpmpp2m_update_kernel, dim3(grid_for(n, 256)), dim3(256), 0,
+                              reinterpret_cast<cudaStream_t>(stream), x, e_c, e_u, gs, x0_prev, alpha_t, sigma_t, c_x,
+                              c_d, w_cur, w_prev, x0_out, x_out, n));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -43,11 +43,13 @@ def resolve_seed(noisy: bool, seed: Optional[int]) -> int:
 
 class Trajectory:
     """One denoising trajectory: its input dict (mutated like the reference does: `x`,
-    `timesteps`) and its history of post-CFG eps (at most 3, plms.py:109-111)."""
+    `timesteps`), its history of post-CFG eps (at most 3, plms.py:109-111) and, for DPM-Solver++(2M), the x0
+    prediction and log-SNR step h of its previous step."""
 
     def __init__(self, input: dict):
         self.input = input
         self.old_eps: List[torch.Tensor] = []
+        self.dpm_prev: Optional[Tuple[torch.Tensor, float]] = None
 
 
 class PLMSBase(object):
@@ -178,6 +180,28 @@ class PLMSBase(object):
             tr.old_eps.append(e_t)
             if len(tr.old_eps) >= 4:
                 tr.old_eps.pop(0)
+
+    @torch.no_grad()
+    def sample_loop(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, k0=0):
+        """The sampling loop of one input dict (plms.py:72-113, ddim.py:63-103) from step k0 (image-to-image) on: the
+        alpha schedule, the host-level inpainting blend and `_step` of this sampler at every step."""
+        b = shape[0]
+        if input["x"] is None:
+            input["x"] = torch.randn(shape, device=self.device)
+        time_range = np.flip(self.ddim_timesteps)
+        total_steps = self.ddim_timesteps.shape[0]
+        alphas = self.alpha_generator_func(len(time_range)) if self.alpha_generator_func is not None else None
+        tr = Trajectory(input)
+        for i in range(k0, len(time_range)):
+            if alphas is not None:
+                self._set_alpha(alphas[i])
+            ts, ts_next = self._timesteps(b, i, time_range)
+            if mask is not None:  # inpainting blend (plms.py:99-103); host-level glue, unused by inference.py
+                assert x0 is not None
+                img_orig = self.diffusion.q_sample(x0, ts)
+                input["x"] = img_orig * mask + (1. - mask) * input["x"]
+            self._step([tr], ts, ts_next, total_steps - i - 1, uc, guidance_scale)
+        return input["x"]
 
     def _timesteps(self, b, i, time_range):
         step = int(time_range[i])

@@ -9,16 +9,19 @@ PLMS updates are `PLMSBase._step_predict` / `_step_finish` on its own trajectori
 and a Multi-instance request merges its latents with `ops.latent_mean` at its own step int(steps * mis), where
 steps is the length of the PLMS schedule (`schedule_steps`: S + 1 for some S, e.g. 31 for S = 30), as there.
 A DDIM request (`sampler="ddim"`) takes `DDIMBase`'s one-evaluation update instead, its eta noise keyed by its own seed
-and the step, so it does not depend on the other requests.  An image-to-image request (`x_init`, `strength`) starts at
-its sampler's step k0 from x_init noised there (`PLMSBase.start_latent`); in lock step it joins the others at step k0,
-so every request ends with the last step.  That per-request machinery is `_RequestState`, which
-`SamplingEngine` (engine.py) drives too: `sample_requests` is the lock-step driver on top of it.  A request with
+and the step, so it does not depend on the other requests; a DPM-Solver++(2M) request (`sampler="dpmpp_2m"`) takes
+`DPMSolverBase`'s one-evaluation multistep update, its x0 history kept on its own trajectory.  An image-to-image request
+(`x_init`, `strength`) starts at its sampler's step k0 from x_init noised there (`PLMSBase.start_latent`); in lock step
+it joins the others at step k0, so every request ends with the last step.  That per-request machinery is
+`_RequestState`, which `SamplingEngine` (engine.py) drives too: `sample_requests` is the lock-step driver on top of it.
+A request with
 `output="image"` gets the image of its latent instead: the drivers decode the latents of the image requests that finish
 together in batched first-stage forwards (`decode_latents`), eagerly and apart from the UNet's caches and graphs.
 
 Contract: each returned latent equals, within floating-point tolerance, what `PLMSSampler.sample()` (input dict,
-mis = 0), `PLMSSamplerInst.sample()` (input list [global, instance_1 .. instance_n]) or `DDIMSampler.sample(eta=,
-seed=)` returns for that request alone on the model in the state it had when `sample_requests` was called.
+mis = 0), `PLMSSamplerInst.sample()` (input list [global, instance_1 .. instance_n]), `DDIMSampler.sample(eta=,
+seed=)` or `DPMSolverSampler.sample()` returns for that request alone on the model in the state it had when
+`sample_requests` was called.
 Afterwards the model's fuser scale and first-conv swap are what a sequential run of the same requests would leave.
 """
 from __future__ import annotations
@@ -35,6 +38,7 @@ from ...modules.attention import GatedSelfAttentionDense
 from ...modules.diffusionmodules.util import make_ddim_timesteps
 from ._plms_common import PLMSBase, Trajectory, resolve_seed
 from .ddim import DDIMBase
+from .dpm_solver import DPMSolverBase
 
 
 @dataclass
@@ -43,10 +47,10 @@ class Request:
     of `PLMSSamplerInst.sample`; `shape`: (B, 4, H, W) of its latent (may be omitted when input x is given);
     `mis`: the Multi-instance fraction (list inputs only).  `S`: the request's step count; `sample_requests` takes it
     from the call (S, if given, must equal it), `SamplingEngine` requires it.  `mask` / `x0` (inpainting) are not
-    supported and raise.  `sampler`: "plms", or "ddim" (`DDIMSampler.sample`: input dict only) with its `eta` and
+    supported and raise.  `sampler`: "plms", "ddim" (`DDIMSampler.sample`: input dict only) with its `eta` and
     `seed` (None at eta > 0: one draw from torch's default CPU generator when `sample_requests` starts or at `submit`,
-    in request order).  `x_init`: a latent of shape (1 or B, C, H, W) to start image-to-image sampling from, which
-    runs the last int(N * strength) of the N schedule steps (the samplers' `x_init` / `strength`); the start noise is
+    in request order), or "dpmpp_2m" (`DPMSolverSampler.sample`: input dict only, eta = 0).  `x_init`: a latent of
+    shape (1 or B, C, H, W) to start image-to-image sampling from, which runs the last int(N * strength) of the N schedule steps (the samplers' `x_init` / `strength`); the start noise is
     keyed by `seed`, drawn as for DDIM when None.  `output`: "latent" (the sampler's latent) or "image" (that latent
     decoded by the driver's `autoencoder` to uint8 (B, 8H, 8W, 3) on the device, `AutoencoderKL.decode_images`)."""
     input: Union[dict, List[dict]]
@@ -66,7 +70,7 @@ class Request:
     output: str = "latent"
 
 
-SAMPLERS = ("plms", "ddim")
+SAMPLERS = ("plms", "ddim", "dpmpp_2m")
 OUTPUTS = ("latent", "image")
 
 
@@ -150,10 +154,12 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
             raise ValueError(f"request {j}: unknown output {req.output!r} (have {', '.join(OUTPUTS)})")
         if not req.eta >= 0:
             raise ValueError(f"request {j}: eta={req.eta} must be >= 0")
-        if req.sampler == "plms" and req.eta != 0:
-            raise ValueError(f"request {j}: eta={req.eta} needs sampler='ddim' (PLMS is deterministic, eta = 0)")
-        if req.sampler == "ddim" and (multi or req.mis != 0):
-            raise ValueError(f"request {j}: DDIM takes one input dict with mis = 0; the Multi-instance Sampler "
+        if req.sampler != "ddim" and req.eta != 0:
+            name = "PLMS" if req.sampler == "plms" else "DPM-Solver++(2M)"
+            raise ValueError(f"request {j}: eta={req.eta} needs sampler='ddim' ({name} is deterministic, eta = 0)")
+        if req.sampler != "plms" and (multi or req.mis != 0):
+            name = "DDIM" if req.sampler == "ddim" else "DPM-Solver++(2M)"
+            raise ValueError(f"request {j}: {name} takes one input dict with mis = 0; the Multi-instance Sampler "
                              "(input list, mis) is PLMS only")
         if req.seed is not None and not 0 <= int(req.seed) < 1 << 64:
             raise ValueError(f"request {j}: seed {req.seed} outside [0, 2^64)")
@@ -203,9 +209,9 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
 
 class _RequestState:
     """One request being sampled by `sample_requests` or `SamplingEngine`: its plan and its own schedule
-    (`make_schedule(S)` of `PLMSBase`, or of `DDIMBase` with the request's eta and seed), what the model was when the
-    request was admitted, and, once started, its trajectories and its position in the schedule.  Both drivers evaluate a
-    request the same way: `begin`, one forward of its trajectories at `fuser_scale()` and `conv_flag(...)`, `advance`
+    (`make_schedule(S)` of `PLMSBase`, of `DDIMBase` with the request's eta and seed, or of `DPMSolverBase`), what the
+    model was when the request was admitted, and, once started, its trajectories and its position in the schedule.
+    Both drivers evaluate a request the same way: `begin`, one forward of its trajectories at `fuser_scale()` and `conv_flag(...)`, `advance`
     with the eps; after the last step `finish` returns its latent."""
 
     def __init__(self, req: Request, plan: RequestPlan, S: int, model, diffusion):
@@ -213,6 +219,9 @@ class _RequestState:
         if req.sampler == "ddim":
             self.base = DDIMBase(diffusion, model)
             self.base.make_schedule(ddim_num_steps=int(S), ddim_eta=float(req.eta))
+        elif req.sampler == "dpmpp_2m":
+            self.base = DPMSolverBase(diffusion, model)
+            self.base.make_schedule(ddim_num_steps=int(S))
         else:
             self.base = PLMSBase(diffusion, model)
             self.base.make_schedule(ddim_num_steps=int(S))

@@ -1,8 +1,7 @@
 """PLMSSampler -- drop-in for ldm/models/diffusion/plms.py (same constructor and `sample`)."""
-import numpy as np
 import torch
 
-from ._plms_common import PLMSBase, Trajectory
+from ._plms_common import PLMSBase
 
 
 class PLMSSampler(PLMSBase):
@@ -24,20 +23,4 @@ class PLMSSampler(PLMSBase):
     @torch.no_grad()
     def plms_sampling(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, k0=0):
         """plms.py:72-113, from step k0 (image-to-image) on."""
-        b = shape[0]
-        if input["x"] is None:
-            input["x"] = torch.randn(shape, device=self.device)
-        time_range = np.flip(self.ddim_timesteps)
-        total_steps = self.ddim_timesteps.shape[0]
-        alphas = self.alpha_generator_func(len(time_range)) if self.alpha_generator_func is not None else None
-        tr = Trajectory(input)
-        for i in range(k0, len(time_range)):
-            if alphas is not None:
-                self._set_alpha(alphas[i])
-            ts, ts_next = self._timesteps(b, i, time_range)
-            if mask is not None:  # inpainting blend (plms.py:99-103); host-level glue, unused by inference.py
-                assert x0 is not None
-                img_orig = self.diffusion.q_sample(x0, ts)
-                input["x"] = img_orig * mask + (1. - mask) * input["x"]
-            self._step([tr], ts, ts_next, total_steps - i - 1, uc, guidance_scale)
-        return input["x"]
+        return self.sample_loop(shape, input, uc, guidance_scale, mask=mask, x0=x0, k0=k0)

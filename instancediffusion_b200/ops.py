@@ -515,6 +515,26 @@ def ddim_update(x: torch.Tensor, e_c: torch.Tensor, e_u: Optional[torch.Tensor],
           "idiff_ddim_update")
 
 
+def dpmpp2m_update(x: torch.Tensor, e_c: torch.Tensor, e_u: Optional[torch.Tensor], gs: float,
+                   x0_prev: Optional[torch.Tensor], alpha_t: float, sigma_t: float, c_x: float, c_d: float,
+                   w_cur: float, w_prev: float, x0_out: Optional[torch.Tensor], x_out: torch.Tensor) -> None:
+    """One DPM-Solver++(2M) step (include/idiff_b200.h idiff_dpmpp2m_update): fp32 contiguous tensors of one size,
+    the scalars computed by the caller (`dpm_solver.dpmpp2m_coefs`).  x0_out receives this step's x0 prediction."""
+    lib = _lib.load()
+    for name, t in (("x", x), ("e_c", e_c), ("e_u", e_u), ("x0_prev", x0_prev), ("x0_out", x0_out),
+                    ("x_out", x_out)):
+        if t is not None:
+            _req(t, torch.float32, name)
+            if t.numel() != x.numel() or not t.is_contiguous():
+                raise _lib.IdiffError(f"dpmpp2m_update: {name} must be contiguous with {x.numel()} elements")
+    if not alpha_t > 0:
+        raise _lib.IdiffError(f"dpmpp2m_update: alpha_t={alpha_t} must be > 0")
+    check(lib.idiff_dpmpp2m_update(x.data_ptr(), e_c.data_ptr(), _ptr(e_u), float(gs), _ptr(x0_prev), float(alpha_t),
+                                   float(sigma_t), float(c_x), float(c_d), float(w_cur), float(w_prev), _ptr(x0_out),
+                                   x_out.data_ptr(), x.numel(), _stream()),
+          "idiff_dpmpp2m_update")
+
+
 def noise_latent(x_init: torch.Tensor, a: float, seed: int, out: torch.Tensor) -> torch.Tensor:
     """The image-to-image start latent (include/idiff_b200.h idiff_noise_latent): out = sqrt(a) * x_init + sqrt(1 - a)
     * z, x_init broadcast over out's leading elements (out.numel() a multiple of x_init.numel()), z a function of (seed,
