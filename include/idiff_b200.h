@@ -259,6 +259,21 @@ int idiff_dpmpp2m_update(const float* x, const float* e_c, const float* e_u, flo
  * ------------------------------------------------------------------------------------------- */
 int idiff_noise_latent(const float* x_init, long n_init, float sqrt_a, float sqrt_1m_a, unsigned long long seed,
                        float* x_out, long n, void* stream);
+/* ---------------------------------------------------------------------------------------------
+ * idiff_encode_posterior: the first-stage encoder's epilogue (autoencoder.py:27-31, distributions.py:24-36), all fp32:
+ *   m      = quant_conv(h)                          (1x1, 8 -> 8: m[o] = bias[o] + sum_k w[o][k] h[k], k in order)
+ *   mean   = m[0:4],  logvar = clamp(m[4:8], -30, 20),  std = exp(0.5 * logvar)
+ *   z      = (mean + std * eps) * scale            (each product and sum rounded on its own)
+ * h (batch, 8, hw) NCHW, the encoder's conv_out; w [8][8], bias [8]; z (batch, 4, hw).  eps of element e = c*hw + p of
+ * image b is a standard normal that depends on (seeds[b], index[b], e) alone: Philox4x32-10 with key
+ * (seed & 0xffffffff, seed >> 32) and counter (c' & 0xffffffff, c' >> 32, index[b], 2), c' = e/4, word e % 4 after
+ * Box-Muller exactly as in idiff_ddim_update.  seeds (uint64) and index (int32, the image's position in its request)
+ * are per-image arrays in device memory, so one launch serves the images of many requests.  Counter word 3 is 0 for
+ * the DDIM eta noise, 1 for the image-to-image start noise and 2 here: one seed keys all three streams.
+ * ------------------------------------------------------------------------------------------- */
+int idiff_encode_posterior(const float* h, const float* w, const float* bias, float scale,
+                           const unsigned long long* seeds, const int* index, float* z, int batch, long hw,
+                           void* stream);
 /* out = mean over `count` latents given as an array of device pointers (plms_instance.py:135) */
 int idiff_latent_mean(const float* const* xs_dev, int count, float* out, long n, void* stream);
 
@@ -272,6 +287,18 @@ int idiff_latent_mean(const float* const* xs_dev, int count, float* out, long n,
  * ------------------------------------------------------------------------------------------- */
 int idiff_conv_in_select(const float* x, const void* w0, const float* b0, const void* w1, const float* b1,
                          const int* flags, void* out, int batch, int h, int w, int cout, void* stream);
+/* ---------------------------------------------------------------------------------------------
+ * idiff_encode_image_in: the first-stage encoder's conv_in (model.py:402; 3x3, padding 1, 3 -> cout channels) on image
+ * bytes, replacing the data loader's arr.astype(np.float32) / 127.5 - 1 and NCHW transpose (dataset/decode_item.py:
+ * 567-568) and the fp32 conv of Encoder.forward:
+ *   out[b, y, x, n] = bias[n] + sum_{ky,kx,c} w[(ky*3 + kx)*3 + c][n] * v[b, y+ky-1, x+kx-1, c]
+ * v = (float)image / 127.5f - 1.0f in fp32 (IEEE division, then the subtraction), zero outside the image (the padding is
+ * in the normalised space); fp32 accumulation in the order (ky, kx, c).  image uint8 NHWC (batch, h, w, 3); w 16-bit
+ * [27, cout] (tap-major, then input channel); bias fp32 [cout]; out 16-bit NHWC [batch*h*w, cout], the tokens the
+ * first ResnetBlock reads.  cout even, <= 512; batch, h <= 65535.
+ * ------------------------------------------------------------------------------------------- */
+int idiff_encode_image_in(const void* image, const void* w, const float* bias, void* out, int batch, int h, int w_,
+                          int cout, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Instance-isolation attention mask, host prep on the GPU

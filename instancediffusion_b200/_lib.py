@@ -83,6 +83,7 @@ SIGNATURES = {
     "idiff_noise_latent": (_i, [_vp, _l, _f, _f, C.c_uint64, _vp, _l, _vp]),
     "idiff_latent_mean": (_i, [_vp, _i, _vp, _l, _vp]),
     "idiff_conv_in_select": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "idiff_encode_image_in": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "idiff_timestep_embedding": (_i, [_vp, _vp, _i, _i, _vp]),
     "idiff_silu_f16": (_i, [_vp, _vp, _l, _vp]),
     "idiff_segs_inconv": (_i, [_vp, C.POINTER(C.c_long), _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
@@ -94,6 +95,7 @@ SIGNATURES = {
     "idiff_vae_latent_in": (_i, [_vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp]),
     "idiff_softmax_rows": (_i, [_vp, _i, _i, _l, _vp]),
     "idiff_decode_to_image": (_i, [_vp, _i, _vp, _i, _l, _vp]),
+    "idiff_encode_posterior": (_i, [_vp, _vp, _vp, _f, _vp, _vp, _vp, _i, _l, _vp]),
     "idiff_embed_tokens": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "idiff_causal_attention_small": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
 }

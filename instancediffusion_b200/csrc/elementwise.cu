@@ -1,6 +1,7 @@
 // HBM-bound helpers of the sampling hot path (ScaleU lives in scaleu.cu): layout
 // conversion, nearest-2x upsample, stride-2 im2col, UniFusion Fourier embedder, timestep
-// embedding and the fused PLMS sampler update.  Reference citations are at each kernel.
+// embedding, the fused sampler updates and the 3x3 convs of few input channels (the UNet's
+// conv_in, the first-stage encoder's conv_in on image bytes).  Reference citations are at each kernel.
 #include "../../include/idiff_b200.h"
 #include "common.cuh"
 #include "host.cuh"
@@ -283,64 +284,95 @@ __global__ void latent_mean_kernel(const float* const* __restrict__ xs, int coun
 }
 
 // ---------------------------------------------------------------------------------------------
-// input conv of the UNet (openaimodel.py:469-480) with the conv chosen per image: 3x3, padding 1,
-// 4 -> cout channels.  One CTA per CONV_IN_ROWS output rows of one image, one thread per channel
-// pair: the thread keeps its 2 x 36 weights in registers and walks the rows, reading the 3x3x4
-// neighbourhood of each pixel from a shared tile of storage-rounded inputs.  One row per CTA: a
-// 2-image 64x64 forward then launches 128 CTAs, enough to spread over the SMs.
+// 3x3, padding-1 convolutions from CIN <= 4 input channels to cout channels in fp32 FMAs: the UNet's input conv
+// (openaimodel.py:469-480) with the conv chosen per image, and the first-stage encoder's conv_in read straight from
+// image bytes (model.py:402).  A CTA computes n pixels x0 .. x0+n-1 of output row y of one image.  threadIdx.x is an
+// output channel pair: the thread keeps its 2 x 9*CIN weights in registers and walks pixels threadIdx.y,
+// threadIdx.y + blockDim.y, ... of the segment, reading the 3x3xCIN neighbourhood of each pixel from a shared tile of the
+// three input rows (one float4 per pixel, channels >= CIN unused) that load(iy, ix) fills.  Each output sums its taps
+// in the fixed order (ky, kx, c) however the rows are split, so the result does not depend on the launch shape.
 // ---------------------------------------------------------------------------------------------
-constexpr int CONV_IN_ROWS = 1;
+template <int CIN, class Load>
+IDIFF_DEVICE void conv3x3_small_cin(const Load& load, float4* tile, const h16* __restrict__ w,
+                                     const float* __restrict__ bias, uint32_t* __restrict__ orow, int H, int W, int y,
+                                     int x0, int n, int cout) {
+  const int TW = n + 2;
+  const int tid = threadIdx.y * blockDim.x + threadIdx.x, nthreads = blockDim.x * blockDim.y;
+  for (int i = tid; i < 3 * TW; i += nthreads) {
+    const int iy = y - 1 + i / TW, ix = x0 - 1 + i % TW;
+    tile[i] = (iy >= 0 && iy < H && ix >= 0 && ix < W) ? load(iy, ix) : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  const int c0 = 2 * threadIdx.x;
+  float2 wr[9 * CIN];
+#pragma unroll
+  for (int k = 0; k < 9 * CIN; ++k)
+    wr[k] = unpack_half2(*reinterpret_cast<const uint32_t*>(w + (long)k * cout + c0));
+  const float2 b = *reinterpret_cast<const float2*>(bias + c0);
+  __syncthreads();
+  for (int px = threadIdx.y; px < n; px += blockDim.y) {
+    float a0 = 0.f, a1 = 0.f;
+#pragma unroll
+    for (int ky = 0; ky < 3; ++ky) {
+#pragma unroll
+      for (int kx = 0; kx < 3; ++kx) {
+        const float4 v = tile[ky * TW + px + kx];
+        const float2* wk = wr + (ky * 3 + kx) * CIN;
+        a0 = fmaf(wk[0].x, v.x, a0); a1 = fmaf(wk[0].y, v.x, a1);
+        a0 = fmaf(wk[1].x, v.y, a0); a1 = fmaf(wk[1].y, v.y, a1);
+        a0 = fmaf(wk[2].x, v.z, a0); a1 = fmaf(wk[2].y, v.z, a1);
+        if (CIN == 4) { a0 = fmaf(wk[CIN - 1].x, v.w, a0); a1 = fmaf(wk[CIN - 1].y, v.w, a1); }
+      }
+    }
+    orow[(long)(x0 + px) * (cout / 2) + threadIdx.x] = pack_half2(a0 + b.x, a1 + b.y);
+  }
+}
 
+// The UNet input conv, 4 -> cout, one CTA per output row of one image and one thread per channel pair, so a 2-image
+// 64x64 forward launches 128 CTAs, enough to spread over the SMs.  The input is rounded to the storage type, as the GEMM
+// path read it.
 __global__ void __launch_bounds__(512)
 conv_in_select_kernel(const float* __restrict__ x, const h16* __restrict__ w0, const float* __restrict__ b0,
                       const h16* __restrict__ w1, const float* __restrict__ b1, const int* __restrict__ flags,
                       uint32_t* __restrict__ out, int H, int W, int cout) {
   pdl_launch_dependents();
   pdl_wait();
-  extern __shared__ float4 tile[];  // [(CONV_IN_ROWS + 2) * (W + 2)], channels of one pixel in one float4
-  const int b = blockIdx.y, y0 = blockIdx.x * CONV_IN_ROWS;
-  const int TW = W + 2;
+  extern __shared__ float4 tile[];  // [3 * (W + 2)]
+  const int b = blockIdx.y, y = blockIdx.x;
   const long plane = (long)H * W;
   const float* xb = x + (long)b * 4 * plane;
-  for (int i = threadIdx.x; i < (CONV_IN_ROWS + 2) * TW; i += blockDim.x) {
-    const int iy = y0 - 1 + i / TW, ix = i % TW - 1;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
-      const long p = (long)iy * W + ix;  // x rounded to the storage type, as the GEMM path reads it
-      v = make_float4(h2f(f2h(xb[p])), h2f(f2h(xb[plane + p])), h2f(f2h(xb[2 * plane + p])),
-                      h2f(f2h(xb[3 * plane + p])));
-    }
-    tile[i] = v;
-  }
+  const auto load = [&](int iy, int ix) {
+    const long p = (long)iy * W + ix;
+    return make_float4(h2f(f2h(xb[p])), h2f(f2h(xb[plane + p])), h2f(f2h(xb[2 * plane + p])), h2f(f2h(xb[3 * plane + p])));
+  };
   const bool sd = flags[b] != 0;
-  const h16* w = sd ? w1 : w0;
-  const int c0 = 2 * threadIdx.x;
-  float2 wr[36];
-#pragma unroll
-  for (int k = 0; k < 36; ++k)
-    wr[k] = unpack_half2(*reinterpret_cast<const uint32_t*>(w + (long)k * cout + c0));
-  const float2 bias = *reinterpret_cast<const float2*>((sd ? b1 : b0) + c0);
-  __syncthreads();
-  const int rows = min(CONV_IN_ROWS, H - y0);
-  for (int r = 0; r < rows; ++r) {
-    uint32_t* orow = out + ((long)b * plane + (long)(y0 + r) * W) * (cout / 2) + threadIdx.x;
-    for (int px = 0; px < W; ++px) {
-      float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-      for (int ky = 0; ky < 3; ++ky) {
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) {
-          const float4 v = tile[(r + ky) * TW + px + kx];
-          const float2* wk = wr + (ky * 3 + kx) * 4;
-          a0 = fmaf(wk[0].x, v.x, a0); a1 = fmaf(wk[0].y, v.x, a1);
-          a0 = fmaf(wk[1].x, v.y, a0); a1 = fmaf(wk[1].y, v.y, a1);
-          a0 = fmaf(wk[2].x, v.z, a0); a1 = fmaf(wk[2].y, v.z, a1);
-          a0 = fmaf(wk[3].x, v.w, a0); a1 = fmaf(wk[3].y, v.w, a1);
-        }
-      }
-      orow[(long)px * (cout / 2)] = pack_half2(a0 + bias.x, a1 + bias.y);
-    }
-  }
+  conv3x3_small_cin<4>(load, tile, sd ? w1 : w0, sd ? b1 : b0, out + ((long)b * plane + (long)y * W) * (cout / 2), H, W,
+                       y, 0, W, cout);
+}
+
+// The first-stage encoder's conv_in, 3 -> cout, from uint8 RGB: x = u / 127.5 - 1 in fp32 as the reference's data
+// loader computes it (IEEE division, then the subtraction), zero padding in that normalised space.  A CTA takes
+// IMAGE_IN_SEG pixels of a row with 256 / (cout / 2) pixel lanes: whole 512-pixel rows at cout = 128 would give 64-thread
+// CTAs with 24.7 KB of tile each.
+constexpr int IMAGE_IN_SEG = 128;
+constexpr int IMAGE_IN_THREADS = 256;
+
+IDIFF_DEVICE float image_value(uint32_t u) { return __fsub_rn(__fdiv_rn((float)u, 127.5f), 1.0f); }
+
+__global__ void __launch_bounds__(IMAGE_IN_THREADS)
+encode_image_in_kernel(const uint8_t* __restrict__ img, const h16* __restrict__ w, const float* __restrict__ bias,
+                       uint32_t* __restrict__ out, int H, int W, int cout) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ float4 tile[3 * (IMAGE_IN_SEG + 2)];
+  const int b = blockIdx.z, y = blockIdx.y, x0 = blockIdx.x * IMAGE_IN_SEG;
+  const long plane = (long)H * W;
+  const uint8_t* ib = img + (long)b * plane * 3;
+  const auto load = [&](int iy, int ix) {
+    const uint8_t* p = ib + ((long)iy * W + ix) * 3;
+    return make_float4(image_value(p[0]), image_value(p[1]), image_value(p[2]), 0.f);
+  };
+  conv3x3_small_cin<3>(load, tile, w, bias, out + ((long)b * plane + (long)y * W) * (cout / 2), H, W, y, x0,
+                       min(IMAGE_IN_SEG, W - x0), cout);
 }
 
 __global__ void silu_f16_kernel(const h16* __restrict__ x, h16* __restrict__ y, long n) {
@@ -547,12 +579,27 @@ extern "C" int idiff_conv_in_select(const float* x, const void* w0, const float*
   IDIFF_REQUIRE(x && w0 && b0 && w1 && b1 && flags && out, "idiff_conv_in_select: null pointer argument");
   IDIFF_REQUIRE(batch > 0 && h > 0 && w > 0 && cout > 0 && cout % 2 == 0 && cout <= 1024,
                 "idiff_conv_in_select: bad shape (batch %d, %dx%d, cout %d)", batch, h, w, cout);
-  const size_t smem = sizeof(float4) * (CONV_IN_ROWS + 2) * (w + 2);
+  const size_t smem = sizeof(float4) * 3 * (w + 2);
   IDIFF_REQUIRE(smem <= 48 * 1024, "idiff_conv_in_select: width %d too large", w);
-  dim3 grid((h + CONV_IN_ROWS - 1) / CONV_IN_ROWS, batch);
+  dim3 grid(h, batch);
   IDIFF_CHECK_CUDA(launch_pdl(conv_in_select_kernel, grid, dim3(cout / 2), smem, reinterpret_cast<cudaStream_t>(stream), x,
                               reinterpret_cast<const h16*>(w0), b0, reinterpret_cast<const h16*>(w1), b1, flags,
                               reinterpret_cast<uint32_t*>(out), h, w, cout));
+  IDIFF_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int idiff_encode_image_in(const void* image, const void* w, const float* bias, void* out, int batch, int h,
+                                     int w_, int cout, void* stream) {
+  IDIFF_REQUIRE(image && w && bias && out, "idiff_encode_image_in: null pointer argument");
+  IDIFF_REQUIRE(batch > 0 && h > 0 && w_ > 0 && cout > 0 && cout % 2 == 0 && cout <= 2 * IMAGE_IN_THREADS,
+                "idiff_encode_image_in: bad shape (batch %d, %dx%d, cout %d)", batch, h, w_, cout);
+  IDIFF_REQUIRE(batch <= 65535 && h <= 65535, "idiff_encode_image_in: batch %d / height %d above 65535", batch, h);
+  const dim3 block(cout / 2, IMAGE_IN_THREADS / (cout / 2));
+  const dim3 grid((w_ + IMAGE_IN_SEG - 1) / IMAGE_IN_SEG, h, batch);
+  IDIFF_CHECK_CUDA(launch_pdl(encode_image_in_kernel, grid, block, 0, reinterpret_cast<cudaStream_t>(stream),
+                              reinterpret_cast<const uint8_t*>(image), reinterpret_cast<const h16*>(w), bias,
+                              reinterpret_cast<uint32_t*>(out), h, w_, cout));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

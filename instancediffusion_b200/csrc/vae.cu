@@ -5,7 +5,8 @@
 //   * row softmax of the single-head mid-block attention (AttnBlock, model.py:150-202): the scores of one
 //     image are a [HW, HW] GEMM output (head_dim 512 does not fit the flash kernels' register tiles and the
 //     block runs once per image), normalised in place;
-//   * image epilogue: the decoder's NCHW output to the uint8 NHWC bytes the reference saves (inference.py:122-125).
+//   * image epilogue: the decoder's NCHW output to the uint8 NHWC bytes the reference saves (inference.py:122-125);
+//   * encoder epilogue: quant_conv and the seeded sample of the posterior (autoencoder.py:27-31) in one pass.
 #include "../../include/idiff_b200.h"
 #include "common.cuh"
 #include "host.cuh"
@@ -163,6 +164,67 @@ decode_to_image_kernel(const T* __restrict__ x, uint8_t* __restrict__ out, int B
   }
 }
 
+// One thread per latent channel c of a group of four pixels p0 .. p0+3 of one image: the eight conv_out planes of those
+// pixels in, the mean and logvar rows of quant_conv (1x1, 8 -> 8, fp32 FMAs in input-channel order), the posterior
+// sample out.  The noise of element e = c*hw + p of image b is word e % 4 of Philox4x32-10 at counter (e/4 lo, e/4 hi,
+// index[b], 2) and key (seed lo, seed hi) after Box-Muller, so it depends on (seed, index, e) alone; with hw % 4 == 0
+// one Philox call serves the thread's four pixels.
+__global__ void __launch_bounds__(256)
+encode_posterior_kernel(const float* __restrict__ h, const float* __restrict__ w, const float* __restrict__ bias,
+                        float scale, const unsigned long long* __restrict__ seeds, const int* __restrict__ index,
+                        float* __restrict__ z, int B, long hw) {
+  constexpr int ZC = 4, MC = 2 * ZC;
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ float sw[MC * MC], sb[MC];
+  if (threadIdx.x < MC * MC) sw[threadIdx.x] = w[threadIdx.x];
+  if (threadIdx.x < MC) sb[threadIdx.x] = bias[threadIdx.x];
+  __syncthreads();
+  const long groups = (hw + 3) / 4;
+  const long total = (long)B * ZC * groups;
+  for (long g = (long)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
+    const long bc = g / groups;
+    const int b = (int)(bc / ZC), c = (int)(bc - (long)b * ZC);
+    const long p0 = (g - bc * groups) * 4;
+    const int n = (int)(hw - p0 < 4 ? hw - p0 : 4);
+    const float* hb = h + (long)b * MC * hw + p0;
+    float mean[4], logvar[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) mean[j] = sb[c], logvar[j] = sb[c + ZC];
+#pragma unroll
+    for (int k = 0; k < MC; ++k) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float v = j < n ? hb[k * hw + j] : 0.f;
+        mean[j] = fmaf(sw[c * MC + k], v, mean[j]);
+        logvar[j] = fmaf(sw[(c + ZC) * MC + k], v, logvar[j]);
+      }
+    }
+    const unsigned long long seed = seeds[b];
+    const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+    const uint32_t idx = (uint32_t)index[b];
+    float* zb = z + ((long)b * ZC + c) * hw + p0;
+    long cached = -1;
+    float eps4[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (j >= n) break;
+      const long e = c * hw + p0 + j;
+      if ((e >> 2) != cached) {
+        cached = e >> 2;
+        const uint4 v = philox4x32_10(make_uint4((uint32_t)cached, (uint32_t)((unsigned long long)cached >> 32), idx, 2u), key);
+        box_muller(v.x, v.y, eps4[0], eps4[1]);
+        box_muller(v.z, v.w, eps4[2], eps4[3]);
+      }
+      const int q = (int)(e & 3);  // selected, not indexed, so eps4 stays in registers
+      const float eps = q == 0 ? eps4[0] : q == 1 ? eps4[1] : q == 2 ? eps4[2] : eps4[3];
+      // distributions.py:26-36 then autoencoder.py:31, each operation rounded on its own like the torch expressions
+      const float stdv = expf(__fmul_rn(0.5f, fminf(fmaxf(logvar[j], -30.f), 20.f)));
+      zb[j] = __fmul_rn(__fadd_rn(mean[j], __fmul_rn(stdv, eps)), scale);
+    }
+  }
+}
+
 }  // namespace idiff
 
 extern "C" int idiff_vae_latent_in(const float* z, const float* w, const float* bias, float inv_scale, void* out,
@@ -213,6 +275,20 @@ extern "C" int idiff_decode_to_image(const void* x, int x_fp32, void* out, int b
     IDIFF_CHECK_CUDA(vec ? launch_pdl(decode_to_image_kernel<h16, true>, dim3(blocks), dim3(256), 0, s, xh, o, batch, hw)
                          : launch_pdl(decode_to_image_kernel<h16, false>, dim3(blocks), dim3(256), 0, s, xh, o, batch, hw));
   }
+  IDIFF_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int idiff_encode_posterior(const float* h, const float* w, const float* bias, float scale,
+                                      const unsigned long long* seeds, const int* index, float* z, int batch, long hw,
+                                      void* stream) {
+  using namespace idiff;
+  IDIFF_REQUIRE(h && w && bias && seeds && index && z, "idiff_encode_posterior: null pointer argument");
+  IDIFF_REQUIRE(batch > 0 && hw > 0, "idiff_encode_posterior: bad shape (batch %d, hw %ld)", batch, hw);
+  const long total = (long)batch * 4 * ((hw + 3) / 4);
+  const int blocks = (int)((total + 255) / 256 < num_sms() * 16 ? (total + 255) / 256 : num_sms() * 16);
+  IDIFF_CHECK_CUDA(launch_pdl(encode_posterior_kernel, dim3(blocks), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
+                              h, w, bias, scale, seeds, index, z, batch, hw));
   IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -6,12 +6,17 @@ utils/checkpoint.py:233), with the arithmetic in libidiff_b200.so.
 decode(z) = Decoder(post_quant_conv(z / scale_factor)): the scale, the 1x1 post_quant_conv and the
 NCHW fp32 -> NHWC fp16 conversion are one kernel (idiff_vae_latent_in); everything after it is the GEMM /
 GroupNorm kernels of the UNet (ldm/modules/diffusionmodules/model.py in this package).
+
+encode_images(images, seed) = posterior.sample() * scale_factor of uint8 images: conv_in reads the bytes
+(idiff_encode_image_in), quant_conv and the sample are one kernel (idiff_encode_posterior) whose noise is keyed by
+(seed, image index) instead of drawn from torch's global generator.
 """
 from __future__ import annotations
 
 import torch
 
 from ... import ops
+from .diffusion._plms_common import resolve_seed
 from ..modules._base import PackedModule, f32
 from ..modules.diffusionmodules.model import Decoder, Encoder
 
@@ -36,6 +41,17 @@ class DiagonalGaussianDistribution(object):
         return self.mean
 
 
+def check_images(images, multiple: int = 8) -> None:
+    """uint8 (B, H, W, 3) with B >= 1 and H, W positive multiples of `multiple`, or ValueError."""
+    if not isinstance(images, torch.Tensor) or images.dtype != torch.uint8:
+        raise ValueError(f"images must be a uint8 tensor, got {getattr(images, 'dtype', type(images))}")
+    if images.dim() != 4 or images.shape[-1] != 3 or images.shape[0] < 1:
+        raise ValueError(f"images must be (B, H, W, 3) RGB, got shape {tuple(images.shape)}")
+    H, W = int(images.shape[1]), int(images.shape[2])
+    if H < 1 or W < 1 or H % multiple or W % multiple:
+        raise ValueError(f"image size {H}x{W} is not a positive multiple of {multiple}")
+
+
 class AutoencoderKL(PackedModule):
     def __init__(self, ddconfig, embed_dim, scale_factor=1):
         super().__init__()
@@ -49,8 +65,11 @@ class AutoencoderKL(PackedModule):
 
     def _pack(self):
         zc = self.post_quant_conv.out_channels
+        mc = self.quant_conv.out_channels
         return {"wpq": f32(self.post_quant_conv.weight).reshape(zc, self.embed_dim).contiguous(),
-                "bpq": f32(self.post_quant_conv.bias)}
+                "bpq": f32(self.post_quant_conv.bias),
+                "wq": f32(self.quant_conv.weight).reshape(mc, self.quant_conv.in_channels).contiguous(),
+                "bq": f32(self.quant_conv.bias)}
 
     @torch.no_grad()
     def encode(self, x):
@@ -59,6 +78,29 @@ class AutoencoderKL(PackedModule):
         h = self.encoder(x)
         moments = torch.nn.functional.conv2d(h, self.quant_conv.weight.float(), self.quant_conv.bias.float())
         return DiagonalGaussianDistribution(moments).sample() * self.scale_factor
+
+    @torch.no_grad()
+    def encode_images(self, images, seed=None):
+        """uint8 RGB images (B, H, W, 3) -> fp32 latents (B, 4, H/8, W/8) on the model's device: `encode` of the images
+        normalised as the reference's data loader does (u / 127.5 - 1 as NCHW, dataset/decode_item.py:567-568), that is
+        posterior.sample() * scale_factor, with image b's posterior noise keyed by (seed, b) (include/idiff_b200.h
+        idiff_encode_posterior).  So the latent of an image depends on the image, the seed and b alone, not on what else
+        is encoded with it or before it.  seed: an integer in [0, 2^64), or None for one draw from torch's default CPU
+        generator (`resolve_seed`)."""
+        seed = resolve_seed(True, seed)
+        return self._encode_images(images, [seed] * int(images.shape[0]), list(range(int(images.shape[0]))))
+
+    def _encode_images(self, images, seeds, index):
+        """`encode_images` with a seed and an in-request index per image, so one forward serves the images of many
+        requests (batched.encode_images)."""
+        if self.embed_dim != 4 or self.quant_conv.in_channels != 8:
+            raise NotImplementedError("encode_images supports the shipped 4-channel latent (embed_dim 4, double_z)")
+        check_images(images, 2 ** (self.encoder.num_resolutions - 1))
+        p = self.pk()
+        dev = p["wq"].device
+        h = self.encoder.forward_images(images.to(dev).contiguous())
+        index = torch.tensor([int(i) for i in index], dtype=torch.int32).to(dev)
+        return ops.encode_posterior(h, p["wq"], p["bq"], float(self.scale_factor), ops.seed_array(seeds, dev), index)
 
     @torch.no_grad()
     def decode(self, z):

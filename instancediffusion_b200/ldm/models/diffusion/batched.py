@@ -16,12 +16,16 @@ it joins the others at step k0, so every request ends with the last step.  That 
 `_RequestState`, which `SamplingEngine` (engine.py) drives too: `sample_requests` is the lock-step driver on top of it.
 A request with
 `output="image"` gets the image of its latent instead: the drivers decode the latents of the image requests that finish
-together in batched first-stage forwards (`decode_latents`), eagerly and apart from the UNet's caches and graphs.
+together in batched first-stage forwards (`decode_latents`), eagerly and apart from the UNet's caches and graphs.  A
+request may also start from an image (`init_image`, uint8): the drivers encode the images of the requests that start
+together in batched first-stage forwards (`encode_images`), eagerly, before those requests' start latents, and the
+request then runs as if it had been given x_init = autoencoder.encode_images(init_image, seed=its seed).
 
 Contract: each returned latent equals, within floating-point tolerance, what `PLMSSampler.sample()` (input dict,
 mis = 0), `PLMSSamplerInst.sample()` (input list [global, instance_1 .. instance_n]), `DDIMSampler.sample(eta=,
 seed=)` or `DPMSolverSampler.sample()` returns for that request alone on the model in the state it had when
-`sample_requests` was called.
+`sample_requests` was called; for an `init_image` request, what the same request with x_init =
+`AutoencoderKL.encode_images(init_image, seed=seed)` returns (bit for bit in batch-invariant mode).
 Afterwards the model's fuser scale and first-conv swap are what a sequential run of the same requests would leave.
 """
 from __future__ import annotations
@@ -52,7 +56,11 @@ class Request:
     in request order), or "dpmpp_2m" (`DPMSolverSampler.sample`: input dict only, eta = 0).  `x_init`: a latent of
     shape (1 or B, C, H, W) to start image-to-image sampling from, which runs the last int(N * strength) of the N schedule steps (the samplers' `x_init` / `strength`); the start noise is
     keyed by `seed`, drawn as for DDIM when None.  `output`: "latent" (the sampler's latent) or "image" (that latent
-    decoded by the driver's `autoencoder` to uint8 (B, 8H, 8W, 3) on the device, `AutoencoderKL.decode_images`)."""
+    decoded by the driver's `autoencoder` to uint8 (B, 8H, 8W, 3) on the device, `AutoencoderKL.decode_images`).
+    `init_image`: instead of x_init, uint8 RGB images (1 or B, 8H, 8W, 3) on any device, which the driver's
+    `autoencoder` encodes with the request's seed (`AutoencoderKL.encode_images(init_image, seed=seed)`) into the x_init
+    the request starts from; one image on a B > 1 request is encoded once and broadcast.  The request is not modified:
+    the latent stays with the driver."""
     input: Union[dict, List[dict]]
     uc: Optional[torch.Tensor] = None
     guidance_scale: float = 1.0
@@ -68,6 +76,7 @@ class Request:
     x_init: Optional[torch.Tensor] = None
     strength: float = 1.0
     output: str = "latent"
+    init_image: Optional[torch.Tensor] = None
 
 
 SAMPLERS = ("plms", "ddim", "dpmpp_2m")
@@ -189,20 +198,33 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
             elif t.shape[1] != ctx_len:
                 raise ValueError(f"request {j}: context length {t.shape[1]} differs from {ctx_len}")
         k0 = 0
-        if req.x_init is None:
+        img2img = req.x_init is not None or req.init_image is not None
+        if req.x_init is not None and req.init_image is not None:
+            raise ValueError(f"request {j}: x_init and init_image are exclusive (give the latent or the image)")
+        if not img2img:
             if req.strength != 1:
-                raise ValueError(f"request {j}: strength={req.strength} needs x_init")
+                raise ValueError(f"request {j}: strength={req.strength} needs x_init or init_image")
         else:
             try:
                 k0 = PLMSBase.start_step(steps, req.strength)
             except ValueError as e:
                 raise ValueError(f"request {j}: {e}") from None
+        if req.x_init is not None:
             xs = tuple(req.x_init.shape)
             if len(xs) != 4 or xs[0] not in (1, shape[0]) or xs[1:] != shape[1:]:
                 raise ValueError(f"request {j}: x_init of shape {xs} does not fit the latent {shape} "
                                  "(want (1 or B, C, H, W))")
+        if req.init_image is not None:
+            im = req.init_image
+            if not isinstance(im, torch.Tensor) or im.dtype != torch.uint8:
+                raise ValueError(f"request {j}: init_image must be a uint8 tensor, got "
+                                 f"{getattr(im, 'dtype', type(im).__name__)}")
+            want = (8 * shape[2], 8 * shape[3], 3)
+            if im.dim() != 4 or im.shape[0] not in (1, shape[0]) or tuple(im.shape[1:]) != want:
+                raise ValueError(f"request {j}: init_image of shape {tuple(im.shape)} does not fit the latent {shape} "
+                                 f"(want (1 or B, {want[0]}, {want[1]}, 3): 8x the latent, RGB)")
         cfg = req.uc is not None and req.guidance_scale != 1
-        merge = PLMSBase.mis_merge_step(steps, req.mis, k0, req.x_init is not None) if multi else None
+        merge = PLMSBase.mis_merge_step(steps, req.mis, k0, img2img) if multi else None
         plans.append(RequestPlan(len(ins) if merge is not None else 1, merge, shape[0], cfg, k0))
     return plans
 
@@ -226,7 +248,8 @@ class _RequestState:
             self.base = PLMSBase(diffusion, model)
             self.base.make_schedule(ddim_num_steps=int(S))
         noisy = req.sampler == "ddim" and self.base.ddim_eta > 0
-        self.base.seed = resolve_seed(noisy or req.x_init is not None, req.seed)
+        self.base.seed = resolve_seed(noisy or req.x_init is not None or req.init_image is not None, req.seed)
+        self.x_init = req.x_init  # an init_image request's is set by `encode_init_images` before `start`
         self.time_range = np.flip(self.base.ddim_timesteps)
         self.steps = len(self.time_range)
         self.alphas = req.alpha_generator_func(self.steps) if req.alpha_generator_func is not None else None
@@ -258,8 +281,10 @@ class _RequestState:
         """The trajectories, when the request starts sampling: an image-to-image request's start latent is made here,
         before its first forward."""
         ins = _inputs_of(self.req)
-        if self.req.x_init is not None:
-            img = self.base.start_latent(self.shape, self.req.x_init, self.plan.k0)
+        if self.req.init_image is not None and self.x_init is None:
+            raise RuntimeError("an init_image request starts after `encode_init_images`")
+        if self.x_init is not None:
+            img = self.base.start_latent(self.shape, self.x_init, self.plan.k0)
         elif ins[0].get("x") is None:  # as the samplers: one noise tensor shared by every trajectory
             img = torch.randn(self.shape, device=self.base.device)
         else:
@@ -374,6 +399,17 @@ class _RequestState:
         return out
 
     @staticmethod
+    def encode_init_images(states: Sequence[_RequestState], autoencoder, max_encode_batch: int) -> None:
+        """The x_init of every `init_image` request among `states`, encoded together by `encode_images` on the
+        requests' device, each with its own seed."""
+        enc = [st for st in states if st.req.init_image is not None]
+        if enc:
+            zs = encode_images(autoencoder, [st.req.init_image.to(st.base.device) for st in enc],
+                               [st.base.seed for st in enc], max_encode_batch)
+            for st, z in zip(enc, zs):
+                st.x_init = z
+
+    @staticmethod
     @contextmanager
     def cache_bounds(model, hoist: int, cat: int, graph_pool=None):
         """Within the block, the model's hoisted-tensor caches hold at least `hoist` text / object K/V entries and `cat`
@@ -396,14 +432,42 @@ class _RequestState:
                     delattr(model, k)
 
 
-def check_decode(requests: Sequence[Request], autoencoder, max_decode_batch: int) -> None:
-    """The decode settings of a driver for `requests`: image requests need an autoencoder."""
+def check_decode(requests: Sequence[Request], autoencoder, max_decode_batch: int, max_encode_batch: int = 8) -> None:
+    """The first-stage settings of a driver for `requests`: image outputs and image inputs need an autoencoder."""
     if int(max_decode_batch) <= 0:
         raise ValueError(f"max_decode_batch must be positive, got {max_decode_batch}")
+    if int(max_encode_batch) <= 0:
+        raise ValueError(f"max_encode_batch must be positive, got {max_encode_batch}")
     if autoencoder is None:
         for j, req in enumerate(requests):
             if req.output == "image":
                 raise ValueError(f"request {j}: output='image' needs the driver's autoencoder (autoencoder=None)")
+            if req.init_image is not None:
+                raise ValueError(f"request {j}: init_image needs the driver's autoencoder (autoencoder=None)")
+
+
+def encode_images(autoencoder, images: Sequence[torch.Tensor], seeds: Sequence[int],
+                  max_encode_batch: int) -> List[torch.Tensor]:
+    """The latents of `images` (each uint8 (B_j, H, W, 3), on one device), encoded together: the images of one size
+    are concatenated in order and run through the autoencoder in chunks of at most `max_encode_batch` images, image b of
+    entry j with seed seeds[j] and index b.  One fp32 (B_j, 4, H/8, W/8) latent per entry, in order, each equal to
+    `autoencoder.encode_images(images[j], seed=seeds[j])` (bit for bit in batch-invariant mode)."""
+    out: List[Optional[torch.Tensor]] = [None] * len(images)
+    by_size: Dict[tuple, List[int]] = {}
+    for j, im in enumerate(images):
+        by_size.setdefault(tuple(im.shape[1:]), []).append(j)
+    m = int(max_encode_batch)
+    for js in by_size.values():
+        x = images[js[0]] if len(js) == 1 else torch.cat([images[j] for j in js])
+        seed = [int(seeds[j]) for j in js for _ in range(images[j].shape[0])]
+        index = [b for j in js for b in range(images[j].shape[0])]
+        parts = [autoencoder._encode_images(x[s:s + m], seed[s:s + m], index[s:s + m]) for s in range(0, x.shape[0], m)]
+        z = parts[0] if len(parts) == 1 else torch.cat(parts)
+        start = 0
+        for j in js:
+            out[j] = z[start:start + images[j].shape[0]]
+            start += images[j].shape[0]
+    return out
 
 
 def decode_latents(autoencoder, latents: Sequence[torch.Tensor], max_decode_batch: int) -> List[torch.Tensor]:
@@ -428,12 +492,15 @@ def decode_latents(autoencoder, latents: Sequence[torch.Tensor], max_decode_batc
 
 @torch.no_grad()
 def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], S: int, *,
-                    max_batch: int = 32, autoencoder=None, max_decode_batch: int = 8) -> List[torch.Tensor]:
+                    max_batch: int = 32, autoencoder=None, max_decode_batch: int = 8,
+                    max_encode_batch: int = 8) -> List[torch.Tensor]:
     """Sample every request in `requests` (Request objects or dicts of its fields) with S steps of its sampler; returns
     one latent per request, in order, or for an `output="image"` request its uint8 (B, 8H, 8W, 3) image.  `max_batch`
     bounds the images of one UNet forward.  After the last step the latents of the image requests are decoded
     together by `autoencoder` (an `AutoencoderKL`, required when a request asks for an image), at most
-    `max_decode_batch` images per decoder forward (`decode_latents`).
+    `max_decode_batch` images per decoder forward (`decode_latents`).  Before the first step the `init_image` requests'
+    images are encoded together by `autoencoder`, at most `max_encode_batch` images per encoder forward
+    (`encode_images`).
 
     The per-image fuser scales are those `utils.model.set_alpha_scale` sets (every gated fuser at the request's
     alpha), and the model is left with that function's result for the last alpha of the last request that has an
@@ -443,8 +510,9 @@ def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], 
     from ....utils.model import set_alpha_scale
     reqs = [r if isinstance(r, Request) else Request(**r) for r in requests]
     plans = check_requests(reqs, S, max_batch, diffusion.num_timesteps)
-    check_decode(reqs, autoencoder, max_decode_batch)
+    check_decode(reqs, autoencoder, max_decode_batch, max_encode_batch)
     states = [_RequestState(r, p, S, model, diffusion) for r, p in zip(reqs, plans)]
+    _RequestState.encode_init_images(states, autoencoder, max_encode_batch)
     for st in states:
         st.start()
     steps = states[0].steps

@@ -10,7 +10,10 @@ when the slowest one finishes.  `SamplingEngine` lets requests join and leave be
 
 A request with `output="image"` (the engine built with `autoencoder=`) finishes with its uint8 (B, 8H, 8W, 3) image
 instead of its latent: the image requests that finish in a tick are decoded together in that tick, at most
-`max_decode_batch` images per first-stage forward (`batched.decode_latents`), eagerly, outside the UNet's graphs.
+`max_decode_batch` images per first-stage forward (`batched.decode_latents`), eagerly, outside the UNet's graphs.  A
+request with an `init_image` starts from that image: the `init_image` requests admitted in a tick are encoded together
+in that tick, before their start latents and forwards, at most `max_encode_batch` images per encoder forward
+(`batched.encode_images`), eagerly, outside the UNet's graphs, each with its own seed (drawn at `submit` when None).
 
 A tick gives every live trajectory exactly one UNet evaluation: the one at t of its current step or, for a request
 in the Euler predictor of its first PLMS step, the corrector's evaluation at t_next (so the corrector rides in the
@@ -35,7 +38,8 @@ The engine never calls set_alpha_scale or swaps the model's first conv.
 Contract: each returned latent equals, within floating-point tolerance, what the request's own
 `PLMSSampler.sample()` / `PLMSSamplerInst.sample()` / `DDIMSampler.sample(eta=, seed=)` / `DPMSolverSampler.sample()`
 returns when it runs alone on the model in the state it had at `submit`, whatever else is live and whenever the
-request arrived.
+request arrived; an `init_image` request's equals that of the same request with x_init =
+`AutoencoderKL.encode_images(init_image, seed=seed)`.
 """
 from __future__ import annotations
 
@@ -77,15 +81,17 @@ class SamplingEngine:
     `max_live_images`: bound of the images of the admitted requests (default 4 * max_batch); `buckets`: the padded
     forward sizes (None: no padding); `share_graph_pool`: capture the graphs of the engine's forwards into one
     memory pool instead of a private pool each (see README); `autoencoder`: the `AutoencoderKL` that decodes
-    `output="image"` requests, at most `max_decode_batch` images per decoder forward."""
+    `output="image"` requests, at most `max_decode_batch` images per decoder forward, and encodes the `init_image` of
+    requests, at most `max_encode_batch` images per encoder forward."""
 
     def __init__(self, model, diffusion, *, max_batch: int = 32, max_live_images: Optional[int] = None,
                  buckets: Optional[Sequence[int]] = (2, 4, 8, 16, 24, 32), share_graph_pool: bool = False,
-                 autoencoder=None, max_decode_batch: int = 8):
+                 autoencoder=None, max_decode_batch: int = 8, max_encode_batch: int = 8):
         if int(max_batch) <= 0:
             raise ValueError(f"max_batch must be positive, got {max_batch}")
-        check_decode([], autoencoder, max_decode_batch)
+        check_decode([], autoencoder, max_decode_batch, max_encode_batch)
         self.autoencoder, self.max_decode_batch = autoencoder, int(max_decode_batch)
+        self.max_encode_batch = int(max_encode_batch)
         self.model, self.diffusion = model, diffusion
         self.max_batch = int(max_batch)
         self.max_live_images = 4 * self.max_batch if max_live_images is None else int(max_live_images)
@@ -121,7 +127,7 @@ class SamplingEngine:
         if req.S is None:
             raise ValueError("request.S (the request's step count) is required")
         plan = check_requests([req], int(req.S), self.max_batch, self.diffusion.num_timesteps)[0]
-        check_decode([req], self.autoencoder, self.max_decode_batch)
+        check_decode([req], self.autoencoder, self.max_decode_batch, self.max_encode_batch)
         size = plan.trajectories * plan.rows()
         if size > self.max_live_images:
             raise ValueError(f"request of {size} images (trajectories x images x CFG) exceeds max_live_images="
@@ -143,11 +149,15 @@ class SamplingEngine:
         """One tick: admit, evaluate every live trajectory once, advance; {ticket: latent} of the finished requests
         ({ticket: image} for image requests, decoded together after the tick's forwards)."""
         live_images = sum(st.images() for st in self._live.values())
+        admitted = []
         while self._queue and live_images + self._queue[0][1].images() <= self.max_live_images:
             ticket, st = self._queue.popleft()
-            st.start()
             self._live[ticket] = st
+            admitted.append(st)
             live_images += st.images()
+        _RequestState.encode_init_images(admitted, self.autoencoder, self.max_encode_batch)
+        for st in admitted:
+            st.start()
         if not self._live:
             return {}
         states = list(self._live.values())

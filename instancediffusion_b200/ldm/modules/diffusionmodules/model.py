@@ -10,7 +10,8 @@ as the reference's ldm/modules/diffusionmodules/model.py, with the arithmetic in
                                  directly, transposed, by running the v projection as W_v . x^T (the v bias
                                  moves behind the softmax, whose rows sum to one, into the proj_out bias)
   Upsample / Downsample (42-76)  nearest 2x + conv3x3 ; F.pad(0,1,0,1) + stride-2 conv (im2col operand)
-  Decoder (462-569) / Encoder (368-460)
+  Decoder (462-569) / Encoder (368-460); Encoder.forward_images runs conv_in on uint8 image bytes
+                                 (idiff_encode_image_in) instead of a 64-channel padded copy and a conv GEMM
 
 Internal convention as in the UNet: fp16 token-major activations [B*H*W, C] (== NHWC) from the first
 convolution to the last; the decoder's image leaves as fp32 NCHW straight from the last GEMM's epilogue.
@@ -23,7 +24,7 @@ import torch
 import torch.nn as nn
 
 from .... import ops
-from ....packing import pack_conv1x1, pack_conv3x3
+from ....packing import pack_conv1x1, pack_conv3x3, pack_conv3x3_taps
 from .._base import half, PackedModule, f32, nchw_to_nhwc16, nhwc16_to_nchw, w16
 
 
@@ -260,11 +261,14 @@ class Encoder(PackedModule):
                                         padding=1)
 
     def _pack(self):
-        return {
+        p = {
             "w_in": _pack3x3(self.conv_in, _pad64(self.in_channels)), "b_in": f32(self.conv_in.bias),
             "g_out": f32(self.norm_out.weight), "b_out": f32(self.norm_out.bias),
             "w_out": _pack3x3(self.conv_out), "cb_out": f32(self.conv_out.bias),
         }
+        if self.in_channels == 3:
+            p["w_img"] = pack_conv3x3_taps(self.conv_in.weight.detach().to(half()))
+        return p
 
     @torch.no_grad()
     def forward(self, x):
@@ -272,6 +276,21 @@ class Encoder(PackedModule):
         B, _, H, W = x.shape
         h = ops.nchw_f32_to_nhwc_f16(x.float(), _pad64(self.in_channels))
         h = ops.gemm(h, p["w_in"], p["b_in"], conv=(B, H, W, _pad64(self.in_channels)))
+        return self._encode_tokens(h, B, H, W)
+
+    @torch.no_grad()
+    def forward_images(self, images):
+        """`forward` of uint8 RGB images (B, H, W, 3) on the device, normalised as the reference's data loader does
+        (u / 127.5 - 1, dataset/decode_item.py:567-568): conv_in reads the bytes (ops.encode_image_in)."""
+        if self.in_channels != 3:
+            raise NotImplementedError(f"forward_images needs a 3-channel conv_in (in_channels={self.in_channels})")
+        p = self.pk()
+        B, H, W, _ = images.shape
+        return self._encode_tokens(ops.encode_image_in(images, p["w_img"], p["b_in"]), B, H, W)
+
+    def _encode_tokens(self, h, B, H, W):
+        """conv_in's output tokens [B*H*W, ch] -> conv_out fp32 NCHW (B, 2*z_channels, H/8, W/8)."""
+        p = self.pk()
         for i_level in range(self.num_resolutions):
             lvl = self.down[i_level]
             for i_block in range(self.num_res_blocks):
@@ -285,7 +304,7 @@ class Encoder(PackedModule):
         h = self.mid.attn_1._fwd(h, B, H, W)
         h = self.mid.block_2._fwd(h, B, H, W)
         h = ops.groupnorm(h, p["g_out"], p["b_out"], batch=B, hw=H * W, groups=32, eps=1e-6, silu=True)
-        out = torch.empty((B, self.conv_out.out_channels, H, W), dtype=torch.float32, device=x.device)
+        out = torch.empty((B, self.conv_out.out_channels, H, W), dtype=torch.float32, device=h.device)
         ops.gemm(h, p["w_out"], p["cb_out"], conv=(B, H, W, self.conv_out.in_channels), out_nchw=out)
         return out
 

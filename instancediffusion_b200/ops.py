@@ -595,6 +595,40 @@ def conv_in_select(x: torch.Tensor, w0: torch.Tensor, b0: torch.Tensor, w1: torc
     return out
 
 
+def encode_image_in(image: torch.Tensor, w: torch.Tensor, bias: torch.Tensor,
+                    out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The first-stage encoder's conv_in on image bytes (include/idiff_b200.h idiff_encode_image_in): image uint8 NHWC
+    (B, H, W, 3) contiguous; w 16-bit [27, Cout] (packing.pack_conv3x3_taps); bias fp32 [Cout].  Returns 16-bit NHWC
+    [B*H*W, Cout] of conv(u / 127.5 - 1), the activation the first ResnetBlock reads."""
+    lib = _lib.load()
+    _req(image, torch.uint8, "image")
+    _req(w, HALF, "w")
+    _req(bias, torch.float32, "bias")
+    if image.dim() != 4 or image.shape[-1] != 3 or image.numel() == 0 or not image.is_contiguous():
+        raise _lib.IdiffError(f"encode_image_in: image must be a contiguous non-empty (B, H, W, 3) tensor, got "
+                              f"{tuple(image.shape)}")
+    B, H, W, _ = image.shape
+    cout = w.shape[-1]
+    if w.dim() != 2 or w.shape[0] != 27 or not w.is_contiguous() or bias.numel() != cout or cout % 2 or cout > 512:
+        raise _lib.IdiffError(f"encode_image_in: w {tuple(w.shape)} / bias {tuple(bias.shape)} are not [27, Cout] / "
+                              "[Cout] with Cout even and <= 512")
+    if B > 65535 or H > 65535:
+        raise _lib.IdiffError(f"encode_image_in: batch {B} / height {H} above 65535")
+    for name, t in (("w", w), ("bias", bias)):
+        if t.device != image.device:
+            raise _lib.IdiffError(f"encode_image_in: image on {image.device}, {name} on {t.device}")
+    if out is None:
+        out = torch.empty((B * H * W, cout), dtype=HALF, device=image.device)
+    _req(out, HALF, "out")
+    if tuple(out.shape) != (B * H * W, cout) or not out.is_contiguous():
+        raise _lib.IdiffError(f"encode_image_in: out must be a contiguous {(B * H * W, cout)} tensor")
+    check(_launch("encode_image_in", 2.0 * B * H * W * cout * 27, 1.0 * image.numel() + 2.0 * out.numel(),
+                  lambda: lib.idiff_encode_image_in(image.data_ptr(), w.data_ptr(), bias.data_ptr(), out.data_ptr(), B,
+                                                    H, W, cout, _stream())),
+          "idiff_encode_image_in")
+    return out
+
+
 def silu(x: torch.Tensor) -> torch.Tensor:
     lib = _lib.load()
     _req(x, HALF, "x")
@@ -666,7 +700,7 @@ def seg_tokens(feat: torch.Tensor, null_pos: torch.Tensor, pos: torch.Tensor, se
 
 
 # ------------------------------------------------------------------------------------------------
-# first-stage decoder pieces (csrc/vae.cu)
+# first-stage decoder and encoder pieces (csrc/vae.cu)
 # ------------------------------------------------------------------------------------------------
 def vae_latent_in(z: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, inv_scale: float) -> torch.Tensor:
     """z fp32 (B, C, H, W) -> fp16 NHWC [B*H*W, 64] = post_quant_conv(z * inv_scale), channels >= C zero."""
@@ -712,6 +746,51 @@ def decode_to_image(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
         raise _lib.IdiffError(f"decode_to_image: x on {x.device}, out on {out.device}")
     check(_launch("decode_to_image", 0.0, (x.element_size() + 1.0) * x.numel(), lambda: lib.idiff_decode_to_image(
         x.data_ptr(), int(x.dtype == torch.float32), out.data_ptr(), B, H * W, _stream())), "idiff_decode_to_image")
+    return out
+
+
+def seed_array(seeds, device) -> torch.Tensor:
+    """Seeds in [0, 2^64) as the uint64 words the kernels read (an int64 tensor with the same bits) on `device`."""
+    seeds = [int(s) for s in seeds]
+    for s in seeds:
+        if not 0 <= s < 1 << 64:
+            raise _lib.IdiffError(f"seed {s} outside [0, 2^64)")
+    words = torch.tensor([s - (1 << 64) if s >= 1 << 63 else s for s in seeds], dtype=torch.int64)
+    return words.to(device)
+
+
+def encode_posterior(h: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, scale: float, seeds: torch.Tensor,
+                     index: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The first-stage encoder's epilogue (include/idiff_b200.h idiff_encode_posterior): h fp32 (B, 8, h, w) contiguous
+    (the encoder's conv_out); w fp32 [8, 8] (quant_conv); bias fp32 [8]; seeds the per-image uint64 seeds as int64 words
+    (`seed_array`) and index int32 (B,) each image's position in its request, both on the device.  Returns fp32
+    (B, 4, h, w) = (mean + exp(0.5 clamp(logvar, -30, 20)) * eps) * scale, eps keyed by (seed, index, element)."""
+    lib = _lib.load()
+    _req(h, torch.float32, "h")
+    _req(w, torch.float32, "w")
+    _req(bias, torch.float32, "bias")
+    _req(seeds, torch.int64, "seeds")
+    _req(index, torch.int32, "index")
+    if h.dim() != 4 or h.shape[1] != 8 or h.numel() == 0 or not h.is_contiguous():
+        raise _lib.IdiffError(f"encode_posterior: h must be a contiguous non-empty (B, 8, h, w) tensor, got "
+                              f"{tuple(h.shape)}")
+    B, _, Hh, Ww = h.shape
+    if tuple(w.shape) != (8, 8) or not w.is_contiguous() or bias.numel() != 8:
+        raise _lib.IdiffError(f"encode_posterior: w {tuple(w.shape)} / bias {tuple(bias.shape)} are not [8, 8] / [8]")
+    if seeds.numel() != B or index.numel() != B or not seeds.is_contiguous() or not index.is_contiguous():
+        raise _lib.IdiffError(f"encode_posterior: seeds {tuple(seeds.shape)} and index {tuple(index.shape)} need {B} "
+                              "entries")
+    for name, t in (("w", w), ("bias", bias), ("seeds", seeds), ("index", index)):
+        if t.device != h.device:
+            raise _lib.IdiffError(f"encode_posterior: h on {h.device}, {name} on {t.device}")
+    if out is None:
+        out = torch.empty((B, 4, Hh, Ww), dtype=torch.float32, device=h.device)
+    _req(out, torch.float32, "out")
+    if tuple(out.shape) != (B, 4, Hh, Ww) or not out.is_contiguous():
+        raise _lib.IdiffError(f"encode_posterior: out must be a contiguous {(B, 4, Hh, Ww)} tensor")
+    check(_launch("encode_posterior", 0.0, 4.0 * (h.numel() + out.numel()), lambda: lib.idiff_encode_posterior(
+        h.data_ptr(), w.data_ptr(), bias.data_ptr(), float(scale), seeds.data_ptr(), index.data_ptr(), out.data_ptr(),
+        B, Hh * Ww, _stream())), "idiff_encode_posterior")
     return out
 
 
