@@ -1,4 +1,4 @@
-"""Shared machinery of the two PLMS samplers (plms.py / plms_instance.py of the reference).
+"""The sampling run every sampler shares (plms.py / plms_instance.py / ddim.py of the reference, and DPM-Solver++).
 
 GPU-first restructuring of `p_sample_plms` (plms.py:117-167 == plms_instance.py:162-212):
   * the conditional and unconditional UNet evaluations -- and, during the Multi-instance phase,
@@ -7,12 +7,17 @@ GPU-first restructuring of `p_sample_plms` (plms.py:117-167 == plms_instance.py:
     kernel (idiff_plms_update) instead of ~12 elementwise launches + deepcopy + 4 torch.full;
   * the schedule scalars are host floats taken from the same fp32 buffers the reference reads.
 
-It also holds what every sampler shares for image-to-image sampling (SDEdit, not in the reference): the start step of
-a strength, the noised start latent and the Multi-instance rule for a truncated schedule.
+`SamplingRun` is one request's sampling on one sampler: its trajectories, its start latent, the timesteps, alpha and
+Multi-instance merge of each step and the sampler's update after each evaluation.  The drop-in `sample()` of every
+sampler drives one run (`PLMSBase.sample_loop`); `sample_requests` and `SamplingEngine` (batched.py, engine.py) drive
+many.  A sampler kind is `PLMSBase` or a subclass (`DDIMBase`, `DPMSolverBase`) whose class attributes tell the drivers
+what they ask about it.  Image-to-image sampling (SDEdit, not in the reference) starts a run at the step k0 of a
+strength from x_init noised there.
 """
 from __future__ import annotations
 
-from typing import List, Optional, Tuple
+from dataclasses import dataclass
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -52,8 +57,79 @@ class Trajectory:
         self.dpm_prev: Optional[Tuple[torch.Tensor, float]] = None
 
 
+@dataclass(frozen=True)
+class RequestPlan:
+    """What the step planner needs of a request: trajectories before the merge (1 for plain PLMS), the step
+    before which they merge (None: never), images per trajectory, whether it evaluates cond + uncond and the step it
+    starts at (k0 > 0: image-to-image)."""
+    trajectories: int
+    merge_step: Optional[int]
+    images: int
+    cfg: bool
+    k0: int = 0
+
+    @classmethod
+    def of(cls, inputs: int, mis: Optional[float], steps: int, k0: int, img2img: bool, images: int,
+           cfg: bool) -> RequestPlan:
+        """The plan of a run of `inputs` input dicts at Multi-instance fraction `mis` (None: one input dict, which
+        never merges) over a schedule of `steps` steps from k0."""
+        merge = None if mis is None else PLMSBase.mis_merge_step(steps, mis, k0, img2img)
+        return cls(inputs if merge is not None else 1, merge, images, cfg, k0)
+
+    def live(self, step: int) -> int:
+        """Trajectories evaluated at `step`."""
+        if step < self.k0:
+            return 0
+        return self.trajectories if self.merge_step is not None and step < self.merge_step else 1
+
+    def rows(self) -> int:
+        """Images one trajectory puts into a forward."""
+        return self.images * (2 if self.cfg else 1)
+
+
+def plan_chunks(slots: Sequence[Tuple[int, int]], plans: Sequence[RequestPlan], max_batch: int) -> List[List[Tuple[int, int]]]:
+    """Split (request, trajectory) slots, in order, into forward chunks of at most `max_batch` images.  A
+    trajectory's cond and uncond images stay in one chunk; a trajectory larger than `max_batch` gets a chunk
+    of its own."""
+    chunks, cur, used = [], [], 0
+    for r, k in slots:
+        n = plans[r].rows()
+        if cur and used + n > max_batch:
+            chunks.append(cur)
+            cur, used = [], 0
+        cur.append((r, k))
+        used += n
+    if cur:
+        chunks.append(cur)
+    return chunks
+
+
+def check_init(steps: int, shape, x_init: Optional[torch.Tensor], strength: float, image: bool = False,
+               needs: str = "x_init") -> int:
+    """Validate the image-to-image arguments of a run of latent `shape` over a schedule of `steps` steps; returns its
+    start step k0 (0 without x_init, which needs strength 1).  `image`: the run starts from an image instead, whose
+    latent x_init is not known yet; `needs` names what a strength below 1 needs."""
+    if x_init is None and not image:
+        if strength != 1:
+            raise ValueError(f"strength={strength} needs {needs} (sampling from pure noise is strength 1)")
+        return 0
+    k0 = PLMSBase.start_step(steps, strength)
+    if x_init is not None:
+        shape, got = tuple(shape), tuple(x_init.shape)
+        if len(got) != 4 or got[0] not in (1, shape[0]) or got[1:] != shape[1:]:
+            raise ValueError(f"x_init of shape {got} does not fit the latent {shape} (want (1 or B, C, H, W))")
+    return k0
+
+
 class PLMSBase(object):
+    """The PLMS sampler kind.  The class attributes describe a kind to the drivers: `sampler` is its `Request.sampler`
+    name (batched.SAMPLERS), `title` its name in messages, `eta_allowed` whether eta may be non-zero,
+    `multi_instance` whether it takes the Multi-instance input list and `corrector_first` whether the first step of a
+    run takes two evaluations (the pseudo improved Euler predictor and its corrector, plms.py:146-152)."""
+    sampler, title = "plms", "PLMS"
+    eta_allowed, multi_instance, corrector_first = False, True, True
     seed = 0  # keys the image-to-image start noise (and DDIMBase's eta noise)
+    max_group = None  # trajectories per forward of `sample_loop` (None: all)
 
     def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None):
         super().__init__()
@@ -91,51 +167,98 @@ class PLMSBase(object):
         self.ddim_alphas_prev = a_prev            # float64 ndarray holding fp32 values
         self.ddim_sqrt_one_minus_alphas = torch.sqrt(1. - a)   # fp32, as np.sqrt(1. - ddim_alphas) there
 
+    def noisy(self) -> bool:
+        """Whether the update draws noise (DDIM at eta > 0): such a run resolves a seed even without x_init."""
+        return False
+
     # ------------------------------------------------------------------------------------------
+    # the drop-in samplers
+    # ------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, x_init=None, strength=1.0,
+               seed=None):
+        """plms.py:65-70 on one input dict.  x_init (a latent of shape (1 or B, C, H, W)) starts image-to-image
+        sampling: the run takes the last int(N * strength) of the N steps from x_init noised to the first of them, the
+        noise keyed by `seed` (None: one draw from torch's default CPU generator).  Without x_init this is the
+        reference's sampler."""
+        return self._sample(S, shape, input, uc, guidance_scale, mask, x0, x_init, strength, seed)
+
+    def _sample(self, S, shape, input, uc, guidance_scale, mask, x0, x_init, strength, seed, eta=0., mis=None):
+        """`sample` of every sampler: the schedule of S steps, the image-to-image arguments, the seed, the run."""
+        if not self.multi_instance and not isinstance(input, dict):
+            raise ValueError(f"{type(self).__name__}.sample takes one input dict; the Multi-instance input list is "
+                             "PLMS only (PLMSSamplerInst)")
+        self.make_schedule(ddim_num_steps=S, ddim_eta=eta)
+        k0 = check_init(len(self.ddim_timesteps), shape, x_init, strength)
+        self.seed = resolve_seed(self.noisy() or x_init is not None, seed)
+        return self.sample_loop(shape, input, uc, guidance_scale, mask=mask, x0=x0, k0=k0, x_init=x_init, mis=mis)
+
+    @torch.no_grad()
+    def sample_loop(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, k0=0, x_init=None, mis=None):
+        """One run on the current schedule from step k0 (plms.py:72-113, plms_instance.py:65-158, ddim.py:63-103):
+        `input` is one input dict, or with `mis` the Multi-instance list [global, inst_1 .. inst_n].  Per step: this
+        sampler's alpha and first-conv swap, the run's merge, timesteps and mask / x0 inpainting blend
+        (plms.py:99-103), the forwards of the trajectories and the update, and after the predictor of a first PLMS step
+        the corrector's forwards."""
+        ins = list(input) if mis is not None else [input]
+        steps = len(self.ddim_timesteps)
+        plan = RequestPlan.of(len(ins), mis, steps, k0, x_init is not None, shape[0],
+                              uc is not None and guidance_scale != 1)
+        alphas = self.alpha_generator_func(steps) if self.alpha_generator_func is not None else None
+        run = SamplingRun(self, ins, shape, plan, guidance_scale, alphas, x_init)
+        run.start()
+        while run.i < run.steps:
+            if alphas is not None:  # first, as in the reference's loop, so the device work of a step keeps its order
+                self._set_alpha(alphas[run.i])
+            run.begin(None if mask is None else (mask, x0))
+            run.advance(self._forward(run, uc))
+            if run.pending is not None:
+                run.advance(self._forward(run, uc))
+        return run.finish()
+
     def _set_alpha(self, alpha):
         if self.alpha_generator_func is not None:
             self.set_alpha_scale(self.model, alpha)
             if alpha == 0:
                 self.model.restore_first_conv_from_SD()
 
-    def _eval(self, trajs: List[Trajectory], uc, guidance_scale):
-        """One batched UNet evaluation for all trajectories: returns [(e_cond, e_uncond|None)]."""
-        use_cfg = uc is not None and guidance_scale != 1
-        if hasattr(self.model, "forward_batched"):
+    def _forward(self, run: SamplingRun, uc):
+        """[(e_cond, e_uncond|None)] of the run's trajectories at their inputs: batched forwards of at most `max_group`
+        trajectories, each with its uncond input, or for a model without `forward_batched` one input at a time (the
+        reference's way)."""
+        cfg = run.plan.cfg
+        if not hasattr(self.model, "forward_batched"):
+            res = []
+            for tr in run.trajs:
+                e_c = self.model(tr.input)
+                e_u = self.model(dict(x=tr.input["x"], timesteps=tr.input["timesteps"], context=uc)) if cfg else None
+                res.append((e_c.float(), None if e_u is None else e_u.float()))
+            return res
+        group = len(run.trajs) if self.max_group is None else self.max_group
+        res = []
+        for chunk in plan_chunks([(0, k) for k in range(len(run.trajs))], [run.plan], group * run.plan.rows()):
             inputs = []
-            for tr in trajs:
+            for _, k in chunk:
+                tr = run.trajs[k]
                 inputs.append(tr.input)
-                if use_cfg:
+                if cfg:
                     inputs.append(dict(x=tr.input["x"], timesteps=tr.input["timesteps"], context=uc))
             outs = self.model.forward_batched(inputs)
-            if use_cfg:
-                return [(outs[2 * i], outs[2 * i + 1]) for i in range(len(trajs))]
-            return [(o, None) for o in outs]
-        res = []  # generic model object: evaluate one by one (reference behaviour)
-        for tr in trajs:
-            e_c = self.model(tr.input)
-            e_u = self.model(dict(x=tr.input["x"], timesteps=tr.input["timesteps"], context=uc)) if use_cfg else None
-            res.append((e_c.float(), None if e_u is None else e_u.float()))
+            res += [(outs[2 * j], outs[2 * j + 1]) for j in range(len(chunk))] if cfg else [(o, None) for o in outs]
         return res
 
-    def _step(self, trajs: List[Trajectory], ts, ts_next, index, uc, guidance_scale):
-        """p_sample_plms for every trajectory in `trajs` (they share the step index)."""
-        for tr in trajs:
-            tr.input["timesteps"] = ts
-        evals = self._eval(trajs, uc, guidance_scale)
-        pending = self._step_predict(trajs, evals, ts_next, index, guidance_scale)
-        if pending is not None:
-            evals = self._eval(trajs, uc, guidance_scale)
-        self._step_finish(trajs, evals, pending, index, guidance_scale)
-
+    # ------------------------------------------------------------------------------------------
+    # the update of a step
+    # ------------------------------------------------------------------------------------------
     def _coefs(self, index):
         return (float(self.ddim_alphas[index]), float(np.float32(self.ddim_alphas_prev[index])),
                 float(self.ddim_sqrt_one_minus_alphas[index]))
 
     def _step_predict(self, trajs: List[Trajectory], evals, ts_next, index, guidance_scale):
-        """First half of `_step` after the evaluation at t.  Trajectories without eps history take the pseudo
-        improved Euler predictor (plms.py:146-152): their inputs move to (x_pred, t_next) and the returned state
-        is finished by `_step_finish` with a second evaluation.  Returns None when one evaluation suffices."""
+        """The update after the evaluation at t of a step of a `corrector_first` kind.  Trajectories without eps
+        history take the pseudo improved Euler predictor (plms.py:146-152): their inputs move to (x_pred, t_next) and
+        the returned state is finished by `_step_finish` with a second evaluation.  Returns None when one evaluation
+        suffices."""
         first = [tr for tr in trajs if len(tr.old_eps) == 0]
         if not first:
             return None
@@ -155,7 +278,7 @@ class PLMSBase(object):
         return x0s, e_ts
 
     def _step_finish(self, trajs: List[Trajectory], evals, pending, index, guidance_scale):
-        """Second half of `_step`: the corrector after the predictor's evaluation at t_next (`pending` from
+        """The update that ends a step: the corrector after the predictor's evaluation at t_next (`pending` from
         `_step_predict`) or the Adams-Bashforth update, then the eps history."""
         a_t, a_prev, s1m = self._coefs(index)
         gs = float(guidance_scale)
@@ -180,28 +303,6 @@ class PLMSBase(object):
             tr.old_eps.append(e_t)
             if len(tr.old_eps) >= 4:
                 tr.old_eps.pop(0)
-
-    @torch.no_grad()
-    def sample_loop(self, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, k0=0):
-        """The sampling loop of one input dict (plms.py:72-113, ddim.py:63-103) from step k0 (image-to-image) on: the
-        alpha schedule, the host-level inpainting blend and `_step` of this sampler at every step."""
-        b = shape[0]
-        if input["x"] is None:
-            input["x"] = torch.randn(shape, device=self.device)
-        time_range = np.flip(self.ddim_timesteps)
-        total_steps = self.ddim_timesteps.shape[0]
-        alphas = self.alpha_generator_func(len(time_range)) if self.alpha_generator_func is not None else None
-        tr = Trajectory(input)
-        for i in range(k0, len(time_range)):
-            if alphas is not None:
-                self._set_alpha(alphas[i])
-            ts, ts_next = self._timesteps(b, i, time_range)
-            if mask is not None:  # inpainting blend (plms.py:99-103); host-level glue, unused by inference.py
-                assert x0 is not None
-                img_orig = self.diffusion.q_sample(x0, ts)
-                input["x"] = img_orig * mask + (1. - mask) * input["x"]
-            self._step([tr], ts, ts_next, total_steps - i - 1, uc, guidance_scale)
-        return input["x"]
 
     def _timesteps(self, b, i, time_range):
         step = int(time_range[i])
@@ -232,19 +333,6 @@ class PLMSBase(object):
         merge = int(steps * mis)
         return None if img2img and merge <= k0 else merge
 
-    def check_init(self, shape, x_init, strength) -> int:
-        """Validate the image-to-image arguments of a run of latent `shape` on the current schedule; returns k0
-        (0 without x_init, which needs strength 1)."""
-        if x_init is None:
-            if strength != 1:
-                raise ValueError(f"strength={strength} needs x_init (sampling from pure noise is strength 1)")
-            return 0
-        k0 = self.start_step(len(self.ddim_timesteps), strength)
-        shape, got = tuple(shape), tuple(x_init.shape)
-        if len(got) != 4 or got[0] not in (1, shape[0]) or got[1:] != shape[1:]:
-            raise ValueError(f"x_init of shape {got} does not fit the latent {shape} (want (1 or B, C, H, W))")
-        return k0
-
     def start_latent(self, shape, x_init: torch.Tensor, k0: int) -> torch.Tensor:
         """x_start = sqrt(acp[t0]) * x_init + sqrt(1 - acp[t0]) * z at t0 = time_range[k0], z keyed by `self.seed`
         (ops.noise_latent), x_init broadcast over the batch of `shape`."""
@@ -254,9 +342,85 @@ class PLMSBase(object):
         ops.noise_latent(x_init.to(device=self.device, dtype=torch.float32).contiguous(), a, self.seed, x)
         return x
 
-    def init_run(self, shape, x_init, strength, seed, noisy=False) -> Tuple[int, Optional[torch.Tensor]]:
-        """A sampler's image-to-image set-up: validates, sets `self.seed` (`resolve_seed`: a run draws noise when it
-        has x_init or `noisy` says so) and returns (k0, x_start), x_start None without x_init."""
-        k0 = self.check_init(shape, x_init, strength)
-        self.seed = resolve_seed(noisy or x_init is not None, seed)
-        return k0, None if x_init is None else self.start_latent(shape, x_init, k0)
+
+class SamplingRun:
+    """One request's sampling on `base`, a sampler whose schedule is made and whose `seed` is set: `inputs` (one input
+    dict, or the Multi-instance list [global, inst_1 .. inst_n]) on a latent of `shape`, as `plan` describes it, with
+    the alpha schedule `alphas` (None: none) and, for image-to-image, `x_init`.  A driver calls `start`, then per
+    evaluation `begin`, one evaluation of `trajs` and `advance` with its eps, until `i` reaches `steps`; `finish`
+    returns the latent.  After the predictor of a first PLMS step `pending` is set and the next evaluation is the
+    corrector's, at t_next of the same step."""
+
+    def __init__(self, base: PLMSBase, inputs: List[dict], shape, plan: RequestPlan, guidance_scale: float,
+                 alphas: Optional[Sequence[float]], x_init: Optional[torch.Tensor] = None):
+        self.base, self.ins, self.shape, self.plan = base, inputs, tuple(shape), plan
+        self.gs = float(guidance_scale)
+        self.alphas = alphas
+        self.x_init = x_init
+        self.time_range = np.flip(base.ddim_timesteps)
+        self.steps = len(self.time_range)
+        self.trajs: List[Trajectory] = []
+        self.i = plan.k0       # current step
+        self.pending = None    # predictor state while the corrector's evaluation is due
+        self.ts_next = None
+
+    def start(self):
+        """The trajectories, all from one start latent: x_init noised at k0 (`PLMSBase.start_latent`), else the inputs'
+        x, else fresh noise.  A Multi-instance image-to-image run whose merge falls before its start runs the global
+        trajectory alone."""
+        if self.x_init is not None:
+            img = self.base.start_latent(self.shape, self.x_init, self.plan.k0)
+        elif self.ins[0].get("x") is None:
+            img = torch.randn(self.shape, device=self.base.device)
+        else:
+            img = None
+        if img is not None:
+            for inp in self.ins:
+                inp["x"] = img
+        self.trajs = [Trajectory(inp) for inp in self.ins[:self.plan.trajectories]]
+
+    def merge(self):
+        """Multi-instance merge: the global trajectory continues from the mean of the n+1 latents
+        (plms_instance.py:135).  A single trajectory is left as it is."""
+        if len(self.trajs) > 1:
+            xs = [tr.input["x"].float().contiguous() for tr in self.trajs]
+            merged = torch.empty_like(xs[0])
+            ops.latent_mean(xs, merged)
+            self.trajs[0].input["x"] = merged
+            self.trajs = self.trajs[:1]
+
+    def begin(self, blend: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
+        """Before an evaluation: the merge due before step i, the timesteps of step i and, with `blend` = (mask, x0),
+        the inpainting blend x = q_sample(x0, t) * mask + (1 - mask) * x -- unless the evaluation is the corrector's
+        of a first PLMS step (the predictor left the inputs at t_next)."""
+        if self.pending is None:
+            if self.plan.merge_step == self.i:
+                self.merge()
+            ts, self.ts_next = self.base._timesteps(self.plan.images, self.i, self.time_range)
+            for tr in self.trajs:
+                tr.input["timesteps"] = ts
+            if blend is not None:
+                mask, x0 = blend
+                assert x0 is not None
+                img_orig = self.base.diffusion.q_sample(x0, ts)
+                for tr in self.trajs:
+                    tr.input["x"] = img_orig * mask + (1. - mask) * tr.input["x"]
+
+    def advance(self, evals):
+        """Advance by an evaluation's [(e_c, e_u|None)] per trajectory: the predictor of a first PLMS step, which
+        leaves `pending` set until the corrector's evaluation, or the corrector or a plain step, which moves to step
+        i + 1."""
+        index = self.steps - self.i - 1
+        pending, self.pending = self.pending, None
+        if pending is None and self.base.corrector_first:
+            self.pending = self.base._step_predict(self.trajs, evals, self.ts_next, index, self.gs)
+            if self.pending is not None:
+                return
+        self.base._step_finish(self.trajs, evals, pending, index, self.gs)
+        self.i += 1
+
+    def finish(self) -> torch.Tensor:
+        """The latent, after the last step and, for mis = 1, the merge that follows it."""
+        if self.plan.merge_step == self.steps:
+            self.merge()
+        return self.trajs[0].input["x"]

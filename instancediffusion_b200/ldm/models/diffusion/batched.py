@@ -4,18 +4,16 @@ A deployment that gets one layout per user would otherwise run one `sample()` ca
 then has the batch of that one request (cond + uncond of one image: 512 GEMM rows at the 16x16 level against
 128-row tiles).  `sample_requests` evaluates, at every step, the live trajectories of all requests together in
 `forward_batched` chunks of up to `max_batch` images, each image with its own request's fuser scale (alpha
-schedule) and first-conv state.  Per request the arithmetic is that of its own sampler: the history and the
-PLMS updates are `PLMSBase._step_predict` / `_step_finish` on its own trajectories with its own guidance scale,
-and a Multi-instance request merges its latents with `ops.latent_mean` at its own step int(steps * mis), where
-steps is the length of the PLMS schedule (`schedule_steps`: S + 1 for some S, e.g. 31 for S = 30), as there.
-A DDIM request (`sampler="ddim"`) takes `DDIMBase`'s one-evaluation update instead, its eta noise keyed by its own seed
-and the step, so it does not depend on the other requests; a DPM-Solver++(2M) request (`sampler="dpmpp_2m"`) takes
-`DPMSolverBase`'s one-evaluation multistep update, its x0 history kept on its own trajectory.  An image-to-image request
-(`x_init`, `strength`) starts at its sampler's step k0 from x_init noised there (`PLMSBase.start_latent`); in lock step
-it joins the others at step k0, so every request ends with the last step.  That per-request machinery is
-`_RequestState`, which `SamplingEngine` (engine.py) drives too: `sample_requests` is the lock-step driver on top of it.
-A request with
-`output="image"` gets the image of its latent instead: the drivers decode the latents of the image requests that finish
+schedule) and first-conv state.  Per request the arithmetic is that of its own sampler: each request is a
+`SamplingRun` (_plms_common.py), the run its sampler's `sample()` drives, on the sampler kind `SAMPLERS[sampler]`
+(`PLMSBase`, `DDIMBase`, `DPMSolverBase`) with its own guidance scale, seed and Multi-instance merge at its own step
+int(steps * mis), where steps is the length of the schedule (`schedule_steps`: S + 1 for some S, e.g. 31 for S = 30).
+A DDIM request's eta noise is keyed by its own seed and the step, so it does not depend on the other requests.  An
+image-to-image request (`x_init`, `strength`) starts at its sampler's step k0 from x_init noised there; in lock step it
+joins the others at step k0, so every request ends with the last step.  `_RequestState` adds to the run what the
+request drivers need: what the model was at admission and the batched evaluation with per-image fuser scales and
+convs.  `SamplingEngine` (engine.py) drives it too: `sample_requests` is the lock-step driver on top of it.  A request
+with `output="image"` gets the image of its latent instead: the drivers decode the latents of the image requests that finish
 together in batched first-stage forwards (`decode_latents`), eagerly and apart from the UNet's caches and graphs.  A
 request may also start from an image (`init_image`, uint8): the drivers encode the images of the requests that start
 together in batched first-stage forwards (`encode_images`), eagerly, before those requests' start latents, and the
@@ -34,13 +32,11 @@ from contextlib import contextmanager
 from dataclasses import dataclass
 from typing import Callable, Dict, List, Optional, Sequence, Tuple, Union
 
-import numpy as np
 import torch
 
-from .... import ops
 from ...modules.attention import GatedSelfAttentionDense
 from ...modules.diffusionmodules.util import make_ddim_timesteps
-from ._plms_common import PLMSBase, Trajectory, resolve_seed
+from ._plms_common import PLMSBase, RequestPlan, SamplingRun, check_init, plan_chunks, resolve_seed
 from .ddim import DDIMBase
 from .dpm_solver import DPMSolverBase
 
@@ -51,9 +47,9 @@ class Request:
     of `PLMSSamplerInst.sample`; `shape`: (B, 4, H, W) of its latent (may be omitted when input x is given);
     `mis`: the Multi-instance fraction (list inputs only).  `S`: the request's step count; `sample_requests` takes it
     from the call (S, if given, must equal it), `SamplingEngine` requires it.  `mask` / `x0` (inpainting) are not
-    supported and raise.  `sampler`: "plms", "ddim" (`DDIMSampler.sample`: input dict only) with its `eta` and
-    `seed` (None at eta > 0: one draw from torch's default CPU generator when `sample_requests` starts or at `submit`,
-    in request order), or "dpmpp_2m" (`DPMSolverSampler.sample`: input dict only, eta = 0).  `x_init`: a latent of
+    supported and raise.  `sampler`: a name of `SAMPLERS`: "plms", "ddim" (`DDIMSampler.sample`: input dict only)
+    with its `eta` and `seed` (None at eta > 0: one draw from torch's default CPU generator when `sample_requests`
+    starts or at `submit`, in request order), or "dpmpp_2m" (`DPMSolverSampler.sample`: input dict only, eta = 0).  `x_init`: a latent of
     shape (1 or B, C, H, W) to start image-to-image sampling from, which runs the last int(N * strength) of the N schedule steps (the samplers' `x_init` / `strength`); the start noise is
     keyed by `seed`, drawn as for DDIM when None.  `output`: "latent" (the sampler's latent) or "image" (that latent
     decoded by the driver's `autoencoder` to uint8 (B, 8H, 8W, 3) on the device, `AutoencoderKL.decode_images`).
@@ -79,47 +75,8 @@ class Request:
     init_image: Optional[torch.Tensor] = None
 
 
-SAMPLERS = ("plms", "ddim", "dpmpp_2m")
+SAMPLERS = {kind.sampler: kind for kind in (PLMSBase, DDIMBase, DPMSolverBase)}
 OUTPUTS = ("latent", "image")
-
-
-@dataclass(frozen=True)
-class RequestPlan:
-    """What the step planner needs of a request: trajectories before the merge (1 for plain PLMS), the step
-    before which they merge (None: never), images per trajectory, whether it evaluates cond + uncond and the step it
-    starts at (k0 > 0: image-to-image)."""
-    trajectories: int
-    merge_step: Optional[int]
-    images: int
-    cfg: bool
-    k0: int = 0
-
-    def live(self, step: int) -> int:
-        """Trajectories evaluated at `step`."""
-        if step < self.k0:
-            return 0
-        return self.trajectories if self.merge_step is not None and step < self.merge_step else 1
-
-    def rows(self) -> int:
-        """Images one trajectory puts into a forward."""
-        return self.images * (2 if self.cfg else 1)
-
-
-def plan_chunks(slots: Sequence[Tuple[int, int]], plans: Sequence[RequestPlan], max_batch: int) -> List[List[Tuple[int, int]]]:
-    """Split (request, trajectory) slots, in order, into forward chunks of at most `max_batch` images.  A
-    trajectory's cond and uncond images stay in one chunk; a trajectory larger than `max_batch` gets a chunk
-    of its own."""
-    chunks, cur, used = [], [], 0
-    for r, k in slots:
-        n = plans[r].rows()
-        if cur and used + n > max_batch:
-            chunks.append(cur)
-            cur, used = [], 0
-        cur.append((r, k))
-        used += n
-    if cur:
-        chunks.append(cur)
-    return chunks
 
 
 def plan_step(plans: Sequence[RequestPlan], step: int, max_batch: int) -> List[List[Tuple[int, int]]]:
@@ -157,19 +114,20 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
         if req.mask is not None or req.x0 is not None:
             raise ValueError(f"request {j}: mask / x0 inpainting is not supported by sample_requests")
         multi = isinstance(req.input, (list, tuple))
-        if req.sampler not in SAMPLERS:
+        kind = SAMPLERS.get(req.sampler)
+        if kind is None:
             raise ValueError(f"request {j}: unknown sampler {req.sampler!r} (have {', '.join(SAMPLERS)})")
         if req.output not in OUTPUTS:
             raise ValueError(f"request {j}: unknown output {req.output!r} (have {', '.join(OUTPUTS)})")
         if not req.eta >= 0:
             raise ValueError(f"request {j}: eta={req.eta} must be >= 0")
-        if req.sampler != "ddim" and req.eta != 0:
-            name = "PLMS" if req.sampler == "plms" else "DPM-Solver++(2M)"
-            raise ValueError(f"request {j}: eta={req.eta} needs sampler='ddim' ({name} is deterministic, eta = 0)")
-        if req.sampler != "plms" and (multi or req.mis != 0):
-            name = "DDIM" if req.sampler == "ddim" else "DPM-Solver++(2M)"
-            raise ValueError(f"request {j}: {name} takes one input dict with mis = 0; the Multi-instance Sampler "
-                             "(input list, mis) is PLMS only")
+        if req.eta != 0 and not kind.eta_allowed:
+            names = " / ".join(f"sampler={n!r}" for n, k in SAMPLERS.items() if k.eta_allowed)
+            raise ValueError(f"request {j}: eta={req.eta} needs {names} ({kind.title} is deterministic, eta = 0)")
+        if not kind.multi_instance and (multi or req.mis != 0):
+            names = " / ".join(k.title for k in SAMPLERS.values() if k.multi_instance)
+            raise ValueError(f"request {j}: {kind.title} takes one input dict with mis = 0; the Multi-instance Sampler "
+                             f"(input list, mis) is {names} only")
         if req.seed is not None and not 0 <= int(req.seed) < 1 << 64:
             raise ValueError(f"request {j}: seed {req.seed} outside [0, 2^64)")
         if not multi and req.mis != 0:
@@ -197,23 +155,13 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
                 ctx_len = t.shape[1]
             elif t.shape[1] != ctx_len:
                 raise ValueError(f"request {j}: context length {t.shape[1]} differs from {ctx_len}")
-        k0 = 0
-        img2img = req.x_init is not None or req.init_image is not None
         if req.x_init is not None and req.init_image is not None:
             raise ValueError(f"request {j}: x_init and init_image are exclusive (give the latent or the image)")
-        if not img2img:
-            if req.strength != 1:
-                raise ValueError(f"request {j}: strength={req.strength} needs x_init or init_image")
-        else:
-            try:
-                k0 = PLMSBase.start_step(steps, req.strength)
-            except ValueError as e:
-                raise ValueError(f"request {j}: {e}") from None
-        if req.x_init is not None:
-            xs = tuple(req.x_init.shape)
-            if len(xs) != 4 or xs[0] not in (1, shape[0]) or xs[1:] != shape[1:]:
-                raise ValueError(f"request {j}: x_init of shape {xs} does not fit the latent {shape} "
-                                 "(want (1 or B, C, H, W))")
+        try:
+            k0 = check_init(steps, shape, req.x_init, req.strength, image=req.init_image is not None,
+                            needs="x_init or init_image")
+        except ValueError as e:
+            raise ValueError(f"request {j}: {e}") from None
         if req.init_image is not None:
             im = req.init_image
             if not isinstance(im, torch.Tensor) or im.dtype != torch.uint8:
@@ -223,36 +171,30 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
             if im.dim() != 4 or im.shape[0] not in (1, shape[0]) or tuple(im.shape[1:]) != want:
                 raise ValueError(f"request {j}: init_image of shape {tuple(im.shape)} does not fit the latent {shape} "
                                  f"(want (1 or B, {want[0]}, {want[1]}, 3): 8x the latent, RGB)")
-        cfg = req.uc is not None and req.guidance_scale != 1
-        merge = PLMSBase.mis_merge_step(steps, req.mis, k0, img2img) if multi else None
-        plans.append(RequestPlan(len(ins) if merge is not None else 1, merge, shape[0], cfg, k0))
+        img2img = req.x_init is not None or req.init_image is not None
+        plans.append(RequestPlan.of(len(ins), req.mis if multi else None, steps, k0, img2img, shape[0],
+                                    req.uc is not None and req.guidance_scale != 1))
     return plans
 
 
-class _RequestState:
-    """One request being sampled by `sample_requests` or `SamplingEngine`: its plan and its own schedule
-    (`make_schedule(S)` of `PLMSBase`, of `DDIMBase` with the request's eta and seed, or of `DPMSolverBase`), what the
-    model was when the request was admitted, and, once started, its trajectories and its position in the schedule.
-    Both drivers evaluate a request the same way: `begin`, one forward of its trajectories at `fuser_scale()` and `conv_flag(...)`, `advance`
-    with the eps; after the last step `finish` returns its latent."""
+class _RequestState(SamplingRun):
+    """One request being sampled by `sample_requests` or `SamplingEngine`: its `SamplingRun` on its sampler kind with
+    `make_schedule(S)` (and the request's eta) and its seed, and what the model was when the request was admitted.
+    Both drivers evaluate a request the same way: `begin`, one forward of its trajectories at `fuser_scale()` and
+    `conv_flag(...)` (`evaluate`), `advance` with the eps; after the last step `finish` returns its latent.  An
+    `init_image` request's x_init is set by `encode_init_images` before `start`."""
 
     def __init__(self, req: Request, plan: RequestPlan, S: int, model, diffusion):
-        self.req, self.plan = req, plan
-        if req.sampler == "ddim":
-            self.base = DDIMBase(diffusion, model)
-            self.base.make_schedule(ddim_num_steps=int(S), ddim_eta=float(req.eta))
-        elif req.sampler == "dpmpp_2m":
-            self.base = DPMSolverBase(diffusion, model)
-            self.base.make_schedule(ddim_num_steps=int(S))
-        else:
-            self.base = PLMSBase(diffusion, model)
-            self.base.make_schedule(ddim_num_steps=int(S))
-        noisy = req.sampler == "ddim" and self.base.ddim_eta > 0
-        self.base.seed = resolve_seed(noisy or req.x_init is not None or req.init_image is not None, req.seed)
-        self.x_init = req.x_init  # an init_image request's is set by `encode_init_images` before `start`
-        self.time_range = np.flip(self.base.ddim_timesteps)
-        self.steps = len(self.time_range)
-        self.alphas = req.alpha_generator_func(self.steps) if req.alpha_generator_func is not None else None
+        base = SAMPLERS[req.sampler](diffusion, model)
+        base.make_schedule(ddim_num_steps=int(S), ddim_eta=float(req.eta))
+        base.seed = resolve_seed(base.noisy() or req.x_init is not None or req.init_image is not None, req.seed)
+        ins = _inputs_of(req)
+        x = next((i["x"] for i in ins if i.get("x") is not None), None)
+        shape = tuple(x.shape) if x is not None else tuple(req.shape)
+        steps = len(base.ddim_timesteps)
+        alphas = req.alpha_generator_func(steps) if req.alpha_generator_func is not None else None
+        super().__init__(base, list(ins), shape, plan, req.guidance_scale, alphas, req.x_init)
+        self.req = req
         self.scale = 0.0  # without an alpha schedule: the model's fuser scale at admission
         if self.alphas is None:
             fusers = [m for m in model.modules() if isinstance(m, GatedSelfAttentionDense)]
@@ -266,34 +208,13 @@ class _RequestState:
         gti = getattr(model, "grounding_tokenizer_input", None)
         own = gti is None or not getattr(gti, "set", False) or gti.batch in (1, plan.images)
         self.null_input = None if own else gti.get_null_input(batch=plan.images)
-        ins = _inputs_of(req)
-        x = next((i["x"] for i in ins if i.get("x") is not None), None)
-        self.shape = tuple(x.shape) if x is not None else tuple(req.shape)
         self.group = (self.shape[2:], ins[0]["context"].shape[1])
-        self.trajs: List[Trajectory] = []
-        self.gs = float(req.guidance_scale)
         self.reached_zero = False
-        self.i = plan.k0       # current step
-        self.pending = None    # predictor state while the corrector's evaluation is due
-        self.ts_next = None
 
     def start(self):
-        """The trajectories, when the request starts sampling: an image-to-image request's start latent is made here,
-        before its first forward."""
-        ins = _inputs_of(self.req)
         if self.req.init_image is not None and self.x_init is None:
             raise RuntimeError("an init_image request starts after `encode_init_images`")
-        if self.x_init is not None:
-            img = self.base.start_latent(self.shape, self.x_init, self.plan.k0)
-        elif ins[0].get("x") is None:  # as the samplers: one noise tensor shared by every trajectory
-            img = torch.randn(self.shape, device=self.base.device)
-        else:
-            img = None
-        if img is not None:
-            for inp in ins:
-                inp["x"] = img
-        # a Multi-instance image-to-image request whose merge falls before its start runs the global trajectory alone
-        self.trajs = [Trajectory(inp) for inp in ins[:self.plan.trajectories]]
+        super().start()
 
     def images(self) -> int:
         """Images the request puts into an evaluation before its merge."""
@@ -301,30 +222,10 @@ class _RequestState:
 
     def inputs(self) -> List[dict]:
         """Every input dict the request's forwards use: its trajectories and its uncond branch."""
-        ins = list(_inputs_of(self.req))
+        ins = list(self.ins)
         if self.plan.cfg:
             ins.append(dict(context=self.req.uc, grounding_input=self.null_input))
         return ins
-
-    def merge(self):
-        """Multi-instance merge: the global trajectory continues from the mean of the n+1 latents
-        (plms_instance.py:135).  A single trajectory is left as it is."""
-        if len(self.trajs) > 1:
-            xs = [tr.input["x"].float().contiguous() for tr in self.trajs]
-            merged = torch.empty_like(xs[0])
-            ops.latent_mean(xs, merged)
-            self.trajs[0].input["x"] = merged
-            self.trajs = self.trajs[:1]
-
-    def begin(self):
-        """Before an evaluation: the merge due before step i and the timesteps of step i, unless the evaluation is the
-        corrector's of the first PLMS step (the predictor left the inputs at t_next)."""
-        if self.pending is None:
-            if self.plan.merge_step == self.i:
-                self.merge()
-            ts, self.ts_next = self.base._timesteps(self.plan.images, self.i, self.time_range)
-            for tr in self.trajs:
-                tr.input["timesteps"] = ts
 
     def fuser_scale(self) -> float:
         """Fuser scale of step i.  Sets `reached_zero` from the first alpha 0 on: there the request's own sampler
@@ -339,25 +240,6 @@ class _RequestState:
         """Whether the request's images take the SD1.5 conv: the model had it at admission, or the request reached
         alpha 0 and `sd_conv` says the model has that conv to give."""
         return self.restored or (self.reached_zero and sd_conv)
-
-    def advance(self, evals):
-        """Advance by an evaluation's [(e_c, e_u|None)] per trajectory: the predictor of a first PLMS step, which
-        leaves `pending` set until the corrector's evaluation, or the corrector or a plain step, which moves to step
-        i + 1."""
-        index = self.steps - self.i - 1
-        pending, self.pending = self.pending, None
-        if pending is None:
-            self.pending = self.base._step_predict(self.trajs, evals, self.ts_next, index, self.gs)
-            if self.pending is not None:
-                return
-        self.base._step_finish(self.trajs, evals, pending, index, self.gs)
-        self.i += 1
-
-    def finish(self) -> torch.Tensor:
-        """The latent, after the last step and, for mis = 1, the merge that follows it."""
-        if self.plan.merge_step == self.steps:
-            self.merge()
-        return self.trajs[0].input["x"]
 
     @staticmethod
     def evaluate(model, states: Sequence[_RequestState], forwards: Sequence[Tuple[List[Tuple[int, int]], Optional[int]]],
@@ -446,48 +328,41 @@ def check_decode(requests: Sequence[Request], autoencoder, max_decode_batch: int
                 raise ValueError(f"request {j}: init_image needs the driver's autoencoder (autoencoder=None)")
 
 
+def _by_size(tensors: Sequence[torch.Tensor], max_batch: int, fn) -> List[torch.Tensor]:
+    """fn over `tensors` (each (B_j, ...)) together: the tensors of one size are concatenated in order and passed in
+    chunks of at most `max_batch` images as fn(chunk, [(j, b)] of its images); one output per tensor, in order."""
+    out: List[Optional[torch.Tensor]] = [None] * len(tensors)
+    by_size: Dict[tuple, List[int]] = {}
+    for j, t in enumerate(tensors):
+        by_size.setdefault(tuple(t.shape[1:]), []).append(j)
+    m = int(max_batch)
+    for js in by_size.values():
+        x = tensors[js[0]] if len(js) == 1 else torch.cat([tensors[j] for j in js])
+        owners = [(j, b) for j in js for b in range(tensors[j].shape[0])]
+        parts = [fn(x[s:s + m], owners[s:s + m]) for s in range(0, x.shape[0], m)]
+        y = parts[0] if len(parts) == 1 else torch.cat(parts)
+        start = 0
+        for j in js:
+            out[j] = y[start:start + tensors[j].shape[0]]
+            start += tensors[j].shape[0]
+    return out
+
+
 def encode_images(autoencoder, images: Sequence[torch.Tensor], seeds: Sequence[int],
                   max_encode_batch: int) -> List[torch.Tensor]:
     """The latents of `images` (each uint8 (B_j, H, W, 3), on one device), encoded together: the images of one size
     are concatenated in order and run through the autoencoder in chunks of at most `max_encode_batch` images, image b of
     entry j with seed seeds[j] and index b.  One fp32 (B_j, 4, H/8, W/8) latent per entry, in order, each equal to
     `autoencoder.encode_images(images[j], seed=seeds[j])` (bit for bit in batch-invariant mode)."""
-    out: List[Optional[torch.Tensor]] = [None] * len(images)
-    by_size: Dict[tuple, List[int]] = {}
-    for j, im in enumerate(images):
-        by_size.setdefault(tuple(im.shape[1:]), []).append(j)
-    m = int(max_encode_batch)
-    for js in by_size.values():
-        x = images[js[0]] if len(js) == 1 else torch.cat([images[j] for j in js])
-        seed = [int(seeds[j]) for j in js for _ in range(images[j].shape[0])]
-        index = [b for j in js for b in range(images[j].shape[0])]
-        parts = [autoencoder._encode_images(x[s:s + m], seed[s:s + m], index[s:s + m]) for s in range(0, x.shape[0], m)]
-        z = parts[0] if len(parts) == 1 else torch.cat(parts)
-        start = 0
-        for j in js:
-            out[j] = z[start:start + images[j].shape[0]]
-            start += images[j].shape[0]
-    return out
+    return _by_size(images, max_encode_batch, lambda x, owners: autoencoder._encode_images(
+        x, [int(seeds[j]) for j, _ in owners], [b for _, b in owners]))
 
 
 def decode_latents(autoencoder, latents: Sequence[torch.Tensor], max_decode_batch: int) -> List[torch.Tensor]:
     """The images of `latents` (each (B_j, 4, h, w)), decoded together: the latents of one size are concatenated in
     order and run through `autoencoder.decode_images` in chunks of at most `max_decode_batch` images; one uint8
     (B_j, 8h, 8w, 3) tensor per latent, in order."""
-    out: List[Optional[torch.Tensor]] = [None] * len(latents)
-    by_size: Dict[tuple, List[int]] = {}
-    for j, z in enumerate(latents):
-        by_size.setdefault(tuple(z.shape[1:]), []).append(j)
-    m = int(max_decode_batch)
-    for js in by_size.values():
-        z = latents[js[0]] if len(js) == 1 else torch.cat([latents[j] for j in js])
-        parts = [autoencoder.decode_images(z[s:s + m]) for s in range(0, z.shape[0], m)]
-        imgs = parts[0] if len(parts) == 1 else torch.cat(parts)
-        start = 0
-        for j in js:
-            out[j] = imgs[start:start + latents[j].shape[0]]
-            start += latents[j].shape[0]
-    return out
+    return _by_size(latents, max_decode_batch, lambda z, _: autoencoder.decode_images(z))
 
 
 @torch.no_grad()
@@ -517,11 +392,11 @@ def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], 
         st.start()
     steps = states[0].steps
     # the model's hoisted-tensor caches must hold every input and every chunk combination of the run, or each
-    # forward recomputes its text / object K/V: raised for the run.  Image-to-image PLMS requests take the corrector's
-    # evaluation of their first step in forwards of their own at their start step.
+    # forward recomputes its text / object K/V: raised for the run.  Image-to-image requests of a `corrector_first`
+    # kind (PLMS) take the corrector's evaluation of their first step in forwards of their own at their start step.
     chunks = {tuple(c) for i in range(steps) for c in plan_step(plans, i, max_batch)}
     for k0 in {p.k0 for p in plans if p.k0 > 0}:
-        slots = [(r, k) for r, p in enumerate(plans) if p.k0 == k0 and reqs[r].sampler == "plms"
+        slots = [(r, k) for r, p in enumerate(plans) if p.k0 == k0 and states[r].base.corrector_first
                  for k in range(p.live(k0))]
         chunks |= {tuple(c) for c in plan_chunks(slots, plans, max_batch)}
     try:

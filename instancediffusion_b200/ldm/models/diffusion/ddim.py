@@ -1,7 +1,8 @@
 """DDIMSampler -- drop-in for ldm/models/diffusion/ddim.py (same constructor, `make_schedule` and `sample`).
 
-GPU-first restructuring of `p_sample_ddim` (ddim.py:106-131), on the machinery of the PLMS samplers (`PLMSBase`):
-  * the conditional and unconditional UNet evaluations are ONE batched forward (`PLMSBase._eval`) instead of two;
+GPU-first restructuring of `p_sample_ddim` (ddim.py:106-131), on the sampling run of the PLMS samplers
+(`PLMSBase.sample_loop`, `SamplingRun`):
+  * the conditional and unconditional UNet evaluations are ONE batched forward instead of two;
   * classifier-free guidance, the x_0 prediction, the x_{t-1} update and the eta noise are one fused kernel
     (idiff_ddim_update) instead of ~10 elementwise torch ops on the fp32 latent.
 
@@ -18,18 +19,20 @@ Documented differences from the reference:
 """
 from __future__ import annotations
 
-from typing import List, Optional
+from typing import List
 
 import torch
 
 from .... import ops
 from ...modules.diffusionmodules.util import make_ddim_sampling_parameters
-from ._plms_common import PLMSBase, Trajectory, resolve_seed  # noqa: F401 (resolve_seed: batched.py)
+from ._plms_common import PLMSBase, Trajectory
 
 
 class DDIMBase(PLMSBase):
-    """`PLMSBase` with the DDIM update: `make_schedule` keeps the eta sigmas, `_step_predict` has nothing to predict and
-    `_step_finish` is one `ops.ddim_update` per trajectory, its noise keyed by (`self.seed`, index)."""
+    """The DDIM sampler kind: `make_schedule` keeps the eta sigmas and `_step_finish`, the one update of a step, is one
+    `ops.ddim_update` per trajectory, its noise keyed by (`self.seed`, index)."""
+    sampler, title = "ddim", "DDIM"
+    eta_allowed, multi_instance, corrector_first = True, False, False
 
     def make_schedule(self, ddim_num_steps, ddim_discretize="uniform", ddim_eta=0., verbose=False):
         """ddim.py:25-54: the schedule of `PLMSBase.make_schedule` and the sigmas of `ddim_eta` (util.py:73-83)."""
@@ -41,9 +44,8 @@ class DDIMBase(PLMSBase):
             alphacums=self.diffusion.alphas_cumprod.detach().float().cpu(), ddim_timesteps=self.ddim_timesteps,
             eta=self.ddim_eta, verbose=verbose)
 
-    def _step_predict(self, trajs: List[Trajectory], evals, ts_next, index, guidance_scale):
-        """DDIM takes one evaluation per step."""
-        return None
+    def noisy(self) -> bool:
+        return self.ddim_eta > 0
 
     def _step_finish(self, trajs: List[Trajectory], evals, pending, index, guidance_scale):
         """p_sample_ddim (ddim.py:110-131) after the evaluation at t, for every trajectory."""
@@ -58,25 +60,14 @@ class DDIMBase(PLMSBase):
 
 
 class DDIMSampler(DDIMBase):
-    def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None):
-        super().__init__(diffusion, model, schedule, alpha_generator_func, set_alpha_scale)
-
     @torch.no_grad()
     def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, eta=0.0, seed=None,
                x_init=None, strength=1.0):
         """ddim.py:57-60.  `input` is one input dict (there is no Multi-instance DDIM sampler).  eta > 0 adds the
         stochastic term of DDIM, its noise fixed by `seed` (see the module docstring).  x_init / strength start
         image-to-image sampling as in PLMSSampler.sample; `seed` keys that start noise too."""
-        if not isinstance(input, dict):
-            raise ValueError("DDIMSampler.sample takes one input dict; the Multi-instance input list is PLMS only "
-                             "(PLMSSamplerInst)")
-        self.make_schedule(ddim_num_steps=S, ddim_eta=eta)
-        k0, x_start = self.init_run(shape, x_init, strength, seed, noisy=self.ddim_eta > 0)
-        if x_start is not None:
-            input["x"] = x_start
-        return self.ddim_sampling(shape, input, uc, guidance_scale, mask=mask, x0=x0, k0=k0)
+        return self._sample(S, shape, input, uc, guidance_scale, mask, x0, x_init, strength, seed, eta=eta)
 
-    @torch.no_grad()
     def ddim_sampling(self, shape, input, uc, guidance_scale=1, mask=None, x0=None, k0=0):
-        """ddim.py:63-103 (its inpainting blend is ddim.py:94-98), from step k0 (image-to-image) on."""
+        """ddim.py:63-103 (its inpainting blend is ddim.py:94-98), from step k0 on: `PLMSBase.sample_loop`."""
         return self.sample_loop(shape, input, uc, guidance_scale, mask=mask, x0=x0, k0=k0)

@@ -41,12 +41,10 @@ def dpmpp2m_coefs(a_t: float, a_n: float, h_prev: Optional[float]) -> Tuple[floa
 
 
 class DPMSolverBase(PLMSBase):
-    """`PLMSBase` with the DPM-Solver++(2M) update: `_step_predict` has nothing to predict and `_step_finish` is one
-    `ops.dpmpp2m_update` per trajectory, which keeps the step's x0 prediction and h as its `dpm_prev`."""
-
-    def _step_predict(self, trajs: List[Trajectory], evals, ts_next, index, guidance_scale):
-        """DPM-Solver++(2M) takes one evaluation per step."""
-        return None
+    """The DPM-Solver++(2M) sampler kind: `_step_finish`, the one update of a step, is one `ops.dpmpp2m_update` per
+    trajectory, which keeps the step's x0 prediction and h as its `dpm_prev`."""
+    sampler, title = "dpmpp_2m", "DPM-Solver++(2M)"
+    eta_allowed, multi_instance, corrector_first = False, False, False
 
     def _step_finish(self, trajs: List[Trajectory], evals, pending, index, guidance_scale):
         a_t, a_n, _ = self._coefs(index)
@@ -63,21 +61,6 @@ class DPMSolverBase(PLMSBase):
 
 
 class DPMSolverSampler(DPMSolverBase):
-    def __init__(self, diffusion, model, schedule="linear", alpha_generator_func=None, set_alpha_scale=None):
-        super().__init__(diffusion, model, schedule, alpha_generator_func, set_alpha_scale)
-
-    @torch.no_grad()
-    def sample(self, S, shape, input, uc=None, guidance_scale=1, mask=None, x0=None, *, x_init=None, strength=1.0,
-               seed=None):
-        """S steps of DPM-Solver++(2M) on one input dict (there is no Multi-instance DPM-Solver++ sampler), with the
-        alpha schedule, first-conv swap and mask / x0 blend of the other samplers.  x_init / strength start
-        image-to-image sampling as in PLMSSampler.sample, the start noise keyed by `seed`; the first step from there
-        takes D = x0 as every first step does."""
-        if not isinstance(input, dict):
-            raise ValueError("DPMSolverSampler.sample takes one input dict; the Multi-instance input list is PLMS only "
-                             "(PLMSSamplerInst)")
-        self.make_schedule(ddim_num_steps=S)
-        k0, x_start = self.init_run(shape, x_init, strength, seed)
-        if x_start is not None:
-            input["x"] = x_start
-        return self.sample_loop(shape, input, uc, guidance_scale, mask=mask, x0=x0, k0=k0)
+    """S steps of DPM-Solver++(2M) on one input dict (there is no Multi-instance DPM-Solver++ sampler), with the other
+    samplers' constructor and `sample` (`PLMSBase.sample`): the alpha schedule, first-conv swap, mask / x0 blend and
+    x_init / strength / seed.  The first step of an image-to-image run takes D = x0 as every first step does."""

@@ -19,10 +19,9 @@ A tick gives every live trajectory exactly one UNet evaluation: the one at t of 
 in the Euler predictor of its first PLMS step, the corrector's evaluation at t_next (so the corrector rides in the
 next tick with everyone else).  A PLMS request therefore retires after schedule_steps(S) + 1 ticks, a DDIM or
 DPM-Solver++(2M) request (one evaluation per step) after schedule_steps(S).  Each request is a
-`batched._RequestState`, the per-request sampling state that `sample_requests` drives too: its own schedule
-(`make_schedule(S)` of `PLMSBase`, of `DDIMBase` with its eta and seed, or of `DPMSolverBase`), its sampler's
-arithmetic (`_step_predict` / `_step_finish`) and its Multi-instance merge before step int(schedule_steps(S) * mis),
-after the last one for mis = 1.  An image-to-image request (`x_init`, `strength`) starts at its step k0 with the start
+`batched._RequestState`, which `sample_requests` drives too: the `SamplingRun` that the request's own `sample()`
+drives (its sampler kind `batched.SAMPLERS[sampler]` with `make_schedule(S)`, its eta and seed, its Multi-instance
+merge before step int(schedule_steps(S) * mis), after the last one for mis = 1) and what the model was at admission.  An image-to-image request (`x_init`, `strength`) starts at its step k0 with the start
 latent made at admission, before its first forward, and so retires after n_run = schedule_steps(S) - k0 ticks (DDIM,
 DPM-Solver++(2M)) or n_run + 1 (PLMS).  PLMS, DDIM and DPM-Solver++(2M) requests of one latent size and context
 length, and of any strength, share forwards.  The engine adds admission, the grouping of a tick's forwards and

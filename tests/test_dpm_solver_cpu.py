@@ -7,7 +7,6 @@ import os
 import sys
 from dataclasses import replace
 
-import numpy as np
 import pytest
 import torch
 
@@ -20,7 +19,7 @@ from fake_unet import AGEN, FakeUNet, _fresh, _latent_mean, _plms_update, _req  
 from test_img2img_cpu import ALPHA_TYPE, TOL, _eval_fn, _i2i  # noqa: E402
 from test_img2img_cpu import _alone as _alone_other  # noqa: E402
 from instancediffusion_b200 import ops  # noqa: E402
-from instancediffusion_b200.ldm.models.diffusion._plms_common import Trajectory  # noqa: E402
+from instancediffusion_b200.ldm.models.diffusion._plms_common import SamplingRun  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion.batched import (  # noqa: E402
     RequestPlan, _RequestState, check_requests, sample_requests, schedule_steps)
 from instancediffusion_b200.ldm.models.diffusion.ddim import DDIMBase, DDIMSampler  # noqa: E402
@@ -128,23 +127,23 @@ def test_mask_blend(diffusion, torch_kernels, monkeypatch):
 # the first step is DDIM's
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("k0", [0, 4])
-def test_first_step_equals_ddim(diffusion, torch_kernels, k0):
+def test_first_run_step_equals_ddim(diffusion, torch_kernels, k0):
     """x_next with D = x0 is sqrt(a_n) x0 + sqrt(1 - a_n) e: the first step of a run (also one from k0 > 0) equals
     DDIM's at eta = 0.  The second step differs: it adds the correction from the first step's x0."""
     S, gs = 10, 7.5
     req = _req(82, S)
-    N = schedule_steps(S)
     outs = {}
     for cls in (DPMSolverBase, DDIMBase):
         base = cls(diffusion, FakeUNet())
         base.make_schedule(S)
-        tr = Trajectory(dict(_fresh(req).input))
-        time_range = np.flip(base.ddim_timesteps)
+        run = SamplingRun(base, [dict(_fresh(req).input)], (1, 4, 64, 64), RequestPlan(1, None, 1, True, k0), gs, None)
+        run.start()
         xs = []
-        for i in (k0, k0 + 1):
-            ts, ts_next = base._timesteps(1, i, time_range)
-            base._step([tr], ts, ts_next, N - i - 1, req.uc, gs)
-            xs.append(tr.input["x"].clone())
+        for i in (k0, k0 + 1):  # one step of the drop-in samplers' loop
+            run.begin()
+            run.advance(base._forward(run, req.uc))
+            assert run.i == i + 1
+            xs.append(run.trajs[0].input["x"].clone())
         outs[cls] = xs
     (d1, d2), (g1, g2) = outs[DPMSolverBase], outs[DDIMBase]
     assert torch.allclose(d1, g1, **TOL), (d1 - g1).abs().max().item()
