@@ -109,8 +109,6 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_launch_dependents();  // the next kernel's prologue may overlap this kernel (host.cuh launch_pdl)
-  pdl_wait();               // operands come from earlier kernels: nothing above touched global memory
 
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(Cfg::PRODUCER_REGS));
@@ -438,9 +436,8 @@ static int launch_attention(const idiff_attn_args* a, cudaStream_t stream) {
     attr_set = true;
   }
   dim3 grid((a->nq + Cfg::BQ - 1) / Cfg::BQ, a->heads, a->batch);
-  IDIFF_CHECK_CUDA(launch_pdl(attention_kernel<D, MASKED>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, tmQ,
-                              tmK0, tmV0, tmK1, tmV1, p));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(attention_kernel<D, MASKED>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, stream, tmQ,
+                          tmK0, tmV0, tmK1, tmV1, p));
   return 0;
 }
 

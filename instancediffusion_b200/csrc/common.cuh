@@ -24,13 +24,6 @@ namespace idiff {
 
 #define IDIFF_DEVICE __device__ __forceinline__
 
-// Programmatic dependent launch (host.cuh launch_pdl): launch_dependents lets the next kernel in the
-// stream become resident and run its prologue while this one is still working; wait blocks until the
-// previous kernel has completed and its global writes are visible.  Both are no-ops for a kernel
-// launched without the attribute.
-IDIFF_DEVICE void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;\n" ::: "memory"); }
-IDIFF_DEVICE void pdl_wait() { asm volatile("griddepcontrol.wait;\n" ::: "memory"); }
-
 IDIFF_DEVICE uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

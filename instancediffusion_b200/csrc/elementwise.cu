@@ -14,8 +14,6 @@ namespace idiff {
 // ---------------------------------------------------------------------------------------------
 __global__ void nchw_f32_to_nhwc_f16_kernel(const float* __restrict__ x, h16* __restrict__ y, int B,
                                             int C, int HW, int CP) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   const long total = (long)B * HW * CP;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int c = (int)(i % CP);
@@ -27,8 +25,6 @@ __global__ void nchw_f32_to_nhwc_f16_kernel(const float* __restrict__ x, h16* __
 }
 __global__ void nhwc_f16_to_nchw_f32_kernel(const h16* __restrict__ x, float* __restrict__ y, int B,
                                             int C, int HW) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   __shared__ float tile[32][33];
   // grid: (HW/32, C/32, B)
   const int b = blockIdx.z;
@@ -47,8 +43,6 @@ __global__ void nhwc_f16_to_nchw_f32_kernel(const h16* __restrict__ x, float* __
 // F.interpolate(scale_factor=2, mode="nearest") (openaimodel.py:107), NHWC, 8 channels/thread
 __global__ void upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int B, int H, int W,
                                   int CV) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   const long total = (long)B * 4 * H * W * CV;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int cv = (int)(i % CV);
@@ -66,8 +60,6 @@ __global__ void upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict
 // asymmetric F.pad (0,1,0,1) + stride-2 padding-0 convolution (diffusionmodules/model.py:70-74)
 __global__ void im2col_s2_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int B, int H, int W,
                                  int CV, int pad_lo) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   const int Ho = H >> 1, Wo = W >> 1;
   const long total = (long)B * Ho * Wo * 9 * CV;
   const uint4 zero = make_uint4(0, 0, 0, 0);
@@ -96,8 +88,6 @@ fourier_embed_kernel(const float* __restrict__ coords, const float* __restrict__
                      const float* __restrict__ text, const float* __restrict__ null_text,
                      const float* __restrict__ null_pos, h16* __restrict__ out, int D,
                      int text_dim, int out_ld, int mask_mode, int dropped) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   __shared__ float red[8];
   __shared__ float s_mpos;
   const int row = blockIdx.x;
@@ -143,8 +133,6 @@ fourier_embed_kernel(const float* __restrict__ coords, const float* __restrict__
 // timestep_embedding (util.py:160-180): [cos(t f) | sin(t f)], f_k = exp(-ln(1e4) k / half)
 __global__ void timestep_embedding_kernel(const float* __restrict__ t, h16* __restrict__ out, int B,
                                           int dim) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   const int half_dim = dim >> 1;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * half_dim) return;
@@ -164,8 +152,6 @@ __global__ void plms_update_kernel(const float* __restrict__ x, const float* __r
                                    float c1, float c2, float c3, float sqrt_at, float sqrt_aprev,
                                    float sqrt_1m_at, float sqrt_1m_aprev, float* __restrict__ e_out,
                                    float* __restrict__ x_out, long n) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     float e = e_c[i];
     if (e_u) {
@@ -193,8 +179,6 @@ __global__ void ddim_update_kernel(const float* __restrict__ x, const float* __r
                                    const float* __restrict__ e_u, float gs, float sqrt_at, float sqrt_1m_at,
                                    float sqrt_aprev, float sqrt_dir, float sigma, uint2 key, uint32_t index,
                                    float* __restrict__ e_out, float* __restrict__ x_out, long n) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   const long groups = (n + 3) / 4;
   for (long c = (long)blockIdx.x * blockDim.x + threadIdx.x; c < groups; c += (long)gridDim.x * blockDim.x) {
     float z[4] = {0.f, 0.f, 0.f, 0.f};
@@ -230,8 +214,6 @@ __global__ void dpmpp2m_update_kernel(const float* __restrict__ x, const float* 
                                       const float* __restrict__ e_u, float gs, const float* __restrict__ x0_prev,
                                       float alpha_t, float sigma_t, float c_x, float c_d, float w_cur, float w_prev,
                                       float* __restrict__ x0_out, float* __restrict__ x_out, long n) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     float e = e_c[i];
     if (e_u) {
@@ -255,8 +237,6 @@ __global__ void dpmpp2m_update_kernel(const float* __restrict__ x, const float* 
 // noise (word 3 = 0), so one seed can key both.  x_init is broadcast over the batch: element i reads i % n_init.
 __global__ void noise_latent_kernel(const float* __restrict__ x_init, long n_init, float sqrt_a, float sqrt_1m_a,
                                     uint2 key, float* __restrict__ x_out, long n) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   const long groups = (n + 3) / 4;
   for (long c = (long)blockIdx.x * blockDim.x + threadIdx.x; c < groups; c += (long)gridDim.x * blockDim.x) {
     float z[4];
@@ -274,8 +254,6 @@ __global__ void noise_latent_kernel(const float* __restrict__ x_init, long n_ini
 
 __global__ void latent_mean_kernel(const float* const* __restrict__ xs, int count, float* __restrict__ out,
                                    long n) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     float s = 0.f;
     for (int k = 0; k < count; ++k) s += xs[k][i];
@@ -334,8 +312,6 @@ __global__ void __launch_bounds__(512)
 conv_in_select_kernel(const float* __restrict__ x, const h16* __restrict__ w0, const float* __restrict__ b0,
                       const h16* __restrict__ w1, const float* __restrict__ b1, const int* __restrict__ flags,
                       uint32_t* __restrict__ out, int H, int W, int cout) {
-  pdl_launch_dependents();
-  pdl_wait();
   extern __shared__ float4 tile[];  // [3 * (W + 2)]
   const int b = blockIdx.y, y = blockIdx.x;
   const long plane = (long)H * W;
@@ -361,8 +337,6 @@ IDIFF_DEVICE float image_value(uint32_t u) { return __fsub_rn(__fdiv_rn((float)u
 __global__ void __launch_bounds__(IMAGE_IN_THREADS)
 encode_image_in_kernel(const uint8_t* __restrict__ img, const h16* __restrict__ w, const float* __restrict__ bias,
                        uint32_t* __restrict__ out, int H, int W, int cout) {
-  pdl_launch_dependents();
-  pdl_wait();
   __shared__ float4 tile[3 * (IMAGE_IN_SEG + 2)];
   const int b = blockIdx.z, y = blockIdx.y, x0 = blockIdx.x * IMAGE_IN_SEG;
   const long plane = (long)H * W;
@@ -376,17 +350,8 @@ encode_image_in_kernel(const uint8_t* __restrict__ img, const h16* __restrict__ 
 }
 
 __global__ void silu_f16_kernel(const h16* __restrict__ x, h16* __restrict__ y, long n) {
-  pdl_launch_dependents();  // programmatic dependent launch: the next kernel may start its prologue
-  pdl_wait();               // ... and this one touches global memory only after its predecessor finished
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
     y[i] = f2h(silu_f(h2f(x[i])));
-}
-
-static inline int grid_for(long total, int threads) {
-  long g = (total + threads - 1) / threads;
-  if (g > num_sms() * 16) g = num_sms() * 16;
-  if (g < 1) g = 1;
-  return (int)g;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -395,8 +360,6 @@ static inline int grid_for(long total, int threads) {
 // one thread per (b, k, a, c) element of att_masks
 __global__ void boxes_to_attmask_kernel(const float* __restrict__ boxes, const int* __restrict__ counts,
                                         float* __restrict__ att, int B, int K, int S) {
-  pdl_launch_dependents();
-  pdl_wait();
   const long total = (long)B * K * S * S;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int c = (int)(i % S);
@@ -420,8 +383,6 @@ __global__ void boxes_to_attmask_kernel(const float* __restrict__ boxes, const i
 // one thread per (b, token): token < P visual, then 4*K object tokens, then `tail`
 __global__ void attmask_words_kernel(const float* __restrict__ att, const int* __restrict__ active,
                                      uint32_t* __restrict__ mq, uint32_t* __restrict__ mk, int B, int K, int P, int tail) {
-  pdl_launch_dependents();
-  pdl_wait();
   const int NK = P + 4 * K + tail;
   const long total = (long)B * NK;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -454,40 +415,35 @@ extern "C" int idiff_nchw_f32_to_nhwc_f16(const float* x, void* y, int batch, in
                                           void* stream) {
   IDIFF_REQUIRE(x && y && c_pad >= c, "idiff_nchw_f32_to_nhwc_f16: bad arguments");
   const long total = (long)batch * hw * c_pad;
-  IDIFF_CHECK_CUDA(launch_pdl(nchw_f32_to_nhwc_f16_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  x, reinterpret_cast<h16*>(y), batch, c, hw, c_pad));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(nchw_f32_to_nhwc_f16_kernel, dim3(grid_for(total, 256, 16)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  x, reinterpret_cast<h16*>(y), batch, c, hw, c_pad));
   return 0;
 }
 
 extern "C" int idiff_nhwc_f16_to_nchw_f32(const void* x, float* y, int batch, int c, int hw, void* stream) {
   IDIFF_REQUIRE(x && y, "idiff_nhwc_f16_to_nchw_f32: null pointer argument");
   dim3 grid((hw + 31) / 32, (c + 31) / 32, batch);
-  IDIFF_CHECK_CUDA(launch_pdl(nhwc_f16_to_nchw_f32_kernel, dim3(grid), dim3(dim3(32, 8)), 0, reinterpret_cast<cudaStream_t>(stream),  reinterpret_cast<const h16*>(x), y, batch, c, hw));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(nhwc_f16_to_nchw_f32_kernel, dim3(grid), dim3(dim3(32, 8)), 0, reinterpret_cast<cudaStream_t>(stream),  reinterpret_cast<const h16*>(x), y, batch, c, hw));
   return 0;
 }
 
 extern "C" int idiff_upsample_nearest2x(const void* x, void* y, int batch, int h, int w, int c, void* stream) {
   IDIFF_REQUIRE(x && y && c % 8 == 0, "idiff_upsample_nearest2x: bad arguments");
   const long total = (long)batch * 4 * h * w * (c / 8);
-  IDIFF_CHECK_CUDA(launch_pdl(upsample2x_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), batch, h, w, c / 8));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(upsample2x_kernel, dim3(grid_for(total, 256, 16)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), batch, h, w, c / 8));
   return 0;
 }
 
 extern "C" int idiff_im2col_s2(const void* x, void* y, int batch, int h, int w, int c, void* stream) {
   IDIFF_REQUIRE(x && y && c % 8 == 0 && h % 2 == 0 && w % 2 == 0, "idiff_im2col_s2: bad arguments");
   const long total = (long)batch * (h / 2) * (w / 2) * 9 * (c / 8);
-  IDIFF_CHECK_CUDA(launch_pdl(im2col_s2_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), batch, h, w, c / 8, 1));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(im2col_s2_kernel, dim3(grid_for(total, 256, 16)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), batch, h, w, c / 8, 1));
   return 0;
 }
 
 extern "C" int idiff_im2col_s2_pad01(const void* x, void* y, int batch, int h, int w, int c, void* stream) {
   IDIFF_REQUIRE(x && y && c % 8 == 0 && h % 2 == 0 && w % 2 == 0, "idiff_im2col_s2_pad01: bad arguments");
   const long total = (long)batch * (h / 2) * (w / 2) * 9 * (c / 8);
-  IDIFF_CHECK_CUDA(launch_pdl(im2col_s2_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), batch, h, w, c / 8, 0));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(im2col_s2_kernel, dim3(grid_for(total, 256, 16)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), batch, h, w, c / 8, 0));
   return 0;
 }
 
@@ -504,16 +460,14 @@ extern "C" int idiff_fourier_embed(const float* coords, const float* masks, cons
     IDIFF_CHECK_CUDA(cudaMemcpyToSymbol(c_freqs, f, sizeof(f)));
     freqs_set = true;
   }
-  IDIFF_CHECK_CUDA(launch_pdl(fourier_embed_kernel, dim3(rows), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  coords, masks, text, null_text, null_pos, reinterpret_cast<h16*>(out), coord_dim, text ? text_dim : 0, out_ld, mask_mode, dropped));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(fourier_embed_kernel, dim3(rows), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  coords, masks, text, null_text, null_pos, reinterpret_cast<h16*>(out), coord_dim, text ? text_dim : 0, out_ld, mask_mode, dropped));
   return 0;
 }
 
 extern "C" int idiff_timestep_embedding(const float* t, void* out, int batch, int dim, void* stream) {
   IDIFF_REQUIRE(t && out && dim % 2 == 0, "idiff_timestep_embedding: bad arguments");
   const int total = batch * dim / 2;
-  IDIFF_CHECK_CUDA(launch_pdl(timestep_embedding_kernel, dim3((total + 127) / 128), dim3(128), 0, reinterpret_cast<cudaStream_t>(stream),  t, reinterpret_cast<h16*>(out), batch, dim));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(timestep_embedding_kernel, dim3((total + 127) / 128), dim3(128), 0, reinterpret_cast<cudaStream_t>(stream),  t, reinterpret_cast<h16*>(out), batch, dim));
   return 0;
 }
 
@@ -522,8 +476,7 @@ extern "C" int idiff_plms_update(const float* x, const float* e_c, const float* 
                                  float c1, float c2, float c3, float a_t, float a_prev,
                                  float sqrt_one_minus_at, float* e_out, float* x_out, long n, void* stream) {
   IDIFF_REQUIRE(x && e_c && x_out && n > 0, "idiff_plms_update: bad arguments");
-  IDIFF_CHECK_CUDA(launch_pdl(plms_update_kernel, dim3(grid_for(n, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  x, e_c, e_u, gs, old1, old2, old3, c0, c1, c2, c3, sqrtf(a_t), sqrtf(a_prev), sqrt_one_minus_at, sqrtf(1.0f - a_prev), e_out, x_out, n));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(plms_update_kernel, dim3(grid_for(n, 256, 16)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  x, e_c, e_u, gs, old1, old2, old3, c0, c1, c2, c3, sqrtf(a_t), sqrtf(a_prev), sqrt_one_minus_at, sqrtf(1.0f - a_prev), e_out, x_out, n));
   return 0;
 }
 
@@ -537,10 +490,9 @@ extern "C" int idiff_ddim_update(const float* x, const float* e_c, const float* 
   const float sqrt_dir = sqrtf(fmaxf(1.0f - a_prev - sigma * sigma, 0.0f));
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   const long groups = (n + 3) / 4;
-  IDIFF_CHECK_CUDA(launch_pdl(ddim_update_kernel, dim3(grid_for(groups, 256)), dim3(256), 0,
-                              reinterpret_cast<cudaStream_t>(stream), x, e_c, e_u, gs, sqrtf(a_t), sqrtf(1.0f - a_t),
-                              sqrtf(a_prev), sqrt_dir, sigma, key, (uint32_t)index, e_out, x_out, n));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(ddim_update_kernel, dim3(grid_for(groups, 256, 16)), dim3(256), 0,
+                          reinterpret_cast<cudaStream_t>(stream), x, e_c, e_u, gs, sqrtf(a_t), sqrtf(1.0f - a_t),
+                          sqrtf(a_prev), sqrt_dir, sigma, key, (uint32_t)index, e_out, x_out, n));
   return 0;
 }
 
@@ -548,10 +500,9 @@ extern "C" int idiff_dpmpp2m_update(const float* x, const float* e_c, const floa
                                     const float* x0_prev, float alpha_t, float sigma_t, float c_x, float c_d,
                                     float w_cur, float w_prev, float* x0_out, float* x_out, long n, void* stream) {
   IDIFF_REQUIRE(x && e_c && x_out && n > 0 && alpha_t > 0.f, "idiff_dpmpp2m_update: bad arguments");
-  IDIFF_CHECK_CUDA(launch_pdl(dpmpp2m_update_kernel, dim3(grid_for(n, 256)), dim3(256), 0,
-                              reinterpret_cast<cudaStream_t>(stream), x, e_c, e_u, gs, x0_prev, alpha_t, sigma_t, c_x,
-                              c_d, w_cur, w_prev, x0_out, x_out, n));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(dpmpp2m_update_kernel, dim3(grid_for(n, 256, 16)), dim3(256), 0,
+                          reinterpret_cast<cudaStream_t>(stream), x, e_c, e_u, gs, x0_prev, alpha_t, sigma_t, c_x,
+                          c_d, w_cur, w_prev, x0_out, x_out, n));
   return 0;
 }
 
@@ -560,17 +511,15 @@ extern "C" int idiff_noise_latent(const float* x_init, long n_init, float sqrt_a
   IDIFF_REQUIRE(x_init && x_out && n > 0 && n_init > 0 && n % n_init == 0, "idiff_noise_latent: bad arguments");
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   const long groups = (n + 3) / 4;
-  IDIFF_CHECK_CUDA(launch_pdl(noise_latent_kernel, dim3(grid_for(groups, 256)), dim3(256), 0,
-                              reinterpret_cast<cudaStream_t>(stream), x_init, n_init, sqrt_a, sqrt_1m_a, key, x_out,
-                              n));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(noise_latent_kernel, dim3(grid_for(groups, 256, 16)), dim3(256), 0,
+                          reinterpret_cast<cudaStream_t>(stream), x_init, n_init, sqrt_a, sqrt_1m_a, key, x_out,
+                          n));
   return 0;
 }
 
 extern "C" int idiff_latent_mean(const float* const* xs_dev, int count, float* out, long n, void* stream) {
   IDIFF_REQUIRE(xs_dev && out && count > 0, "idiff_latent_mean: bad arguments");
-  IDIFF_CHECK_CUDA(launch_pdl(latent_mean_kernel, dim3(grid_for(n, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), xs_dev, count, out, n));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(latent_mean_kernel, dim3(grid_for(n, 256, 16)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), xs_dev, count, out, n));
   return 0;
 }
 
@@ -582,10 +531,9 @@ extern "C" int idiff_conv_in_select(const float* x, const void* w0, const float*
   const size_t smem = sizeof(float4) * 3 * (w + 2);
   IDIFF_REQUIRE(smem <= 48 * 1024, "idiff_conv_in_select: width %d too large", w);
   dim3 grid(h, batch);
-  IDIFF_CHECK_CUDA(launch_pdl(conv_in_select_kernel, grid, dim3(cout / 2), smem, reinterpret_cast<cudaStream_t>(stream), x,
-                              reinterpret_cast<const h16*>(w0), b0, reinterpret_cast<const h16*>(w1), b1, flags,
-                              reinterpret_cast<uint32_t*>(out), h, w, cout));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(conv_in_select_kernel, grid, dim3(cout / 2), smem, reinterpret_cast<cudaStream_t>(stream), x,
+                          reinterpret_cast<const h16*>(w0), b0, reinterpret_cast<const h16*>(w1), b1, flags,
+                          reinterpret_cast<uint32_t*>(out), h, w, cout));
   return 0;
 }
 
@@ -597,17 +545,15 @@ extern "C" int idiff_encode_image_in(const void* image, const void* w, const flo
   IDIFF_REQUIRE(batch <= 65535 && h <= 65535, "idiff_encode_image_in: batch %d / height %d above 65535", batch, h);
   const dim3 block(cout / 2, IMAGE_IN_THREADS / (cout / 2));
   const dim3 grid((w_ + IMAGE_IN_SEG - 1) / IMAGE_IN_SEG, h, batch);
-  IDIFF_CHECK_CUDA(launch_pdl(encode_image_in_kernel, grid, block, 0, reinterpret_cast<cudaStream_t>(stream),
-                              reinterpret_cast<const uint8_t*>(image), reinterpret_cast<const h16*>(w), bias,
-                              reinterpret_cast<uint32_t*>(out), h, w_, cout));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(encode_image_in_kernel, grid, block, 0, reinterpret_cast<cudaStream_t>(stream),
+                          reinterpret_cast<const uint8_t*>(image), reinterpret_cast<const h16*>(w), bias,
+                          reinterpret_cast<uint32_t*>(out), h, w_, cout));
   return 0;
 }
 
 extern "C" int idiff_silu_f16(const void* x, void* y, long n, void* stream) {
   IDIFF_REQUIRE(x && y && n > 0, "idiff_silu_f16: bad arguments");
-  IDIFF_CHECK_CUDA(launch_pdl(silu_f16_kernel, dim3(grid_for(n, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  reinterpret_cast<const h16*>(x), reinterpret_cast<h16*>(y), n));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(silu_f16_kernel, dim3(grid_for(n, 256, 16)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),  reinterpret_cast<const h16*>(x), reinterpret_cast<h16*>(y), n));
   return 0;
 }
 
@@ -616,9 +562,8 @@ extern "C" int idiff_boxes_to_attmask(const float* boxes, const int* counts, flo
   using namespace idiff;
   IDIFF_REQUIRE(boxes && counts && att_masks && batch > 0 && max_objs > 0 && size > 0, "idiff_boxes_to_attmask: bad arguments");
   const long total = (long)batch * max_objs * size * size;
-  IDIFF_CHECK_CUDA(launch_pdl(boxes_to_attmask_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-                              boxes, counts, att_masks, batch, max_objs, size));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(boxes_to_attmask_kernel, dim3(grid_for(total, 256, 16)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
+                          boxes, counts, att_masks, batch, max_objs, size));
   return 0;
 }
 
@@ -628,9 +573,8 @@ extern "C" int idiff_attmask_words(const float* att_masks, const int* active, vo
   IDIFF_REQUIRE(att_masks && active && mask_q && mask_k, "idiff_attmask_words: null pointer argument");
   IDIFF_REQUIRE(n_objs > 0 && n_objs <= 30 && pixels > 0 && tail >= 0, "idiff_attmask_words: 1..30 instances supported (got %d)", n_objs);
   const long total = (long)batch * (pixels + 4 * n_objs + tail);
-  IDIFF_CHECK_CUDA(launch_pdl(attmask_words_kernel, dim3(grid_for(total, 256)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-                              att_masks, active, reinterpret_cast<uint32_t*>(mask_q), reinterpret_cast<uint32_t*>(mask_k), batch,
-                              n_objs, pixels, tail));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(attmask_words_kernel, dim3(grid_for(total, 256, 16)), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
+                          att_masks, active, reinterpret_cast<uint32_t*>(mask_q), reinterpret_cast<uint32_t*>(mask_k), batch,
+                          n_objs, pixels, tail));
   return 0;
 }

@@ -236,8 +236,6 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_launch_dependents();  // the next kernel's prologue may overlap this kernel (host.cuh launch_pdl)
-  pdl_wait();               // operands come from earlier kernels: nothing above touched global memory
   auto stamp = [&](int slot) {
     if (p.trace) {
       unsigned long long t;
@@ -779,7 +777,6 @@ gemm2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
 static void* g_ws = nullptr;
 static unsigned long long* g_trace = nullptr;
 static long g_ws_bytes = 0;
-static int g_num_sms = 0;
 constexpr long kFlagBytes = 64 * 1024;
 
 static void choose_patch(int H, int W, int* PW, int* PH, int* PB) {
@@ -880,30 +877,25 @@ static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
     if (a->residual && encode_epi_map(&tmR, a->residual, a->N, a->ldr, a, p)) return -1;
   }
 
-  if (g_num_sms == 0) {
-    int dev = 0;
-    IDIFF_CHECK_CUDA(cudaGetDevice(&dev));
-    IDIFF_CHECK_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev));
-  }
+  const int sms = idiff::num_sms();
   // Stream-K needs the fixup workspace (flags in its first 64 KiB, partial tiles after); short-K
   // problems (fixup cost ~ mainloop) and exact multiples of the SM count stay data-parallel.
-  const long ws_need = kFlagBytes + (long)g_num_sms * 128 * BN * sizeof(float);
+  const long ws_need = kFlagBytes + (long)sms * 128 * BN * sizeof(float);
   // per-call scratch (idiff_gemm_args.workspace: one per stream, so concurrent streams never share flags)
   // takes precedence over the process-wide default of idiff_set_gemm_workspace
   void* ws_ptr = a->workspace ? a->workspace : g_ws;
   const long ws_bytes = a->workspace ? a->workspace_bytes : g_ws_bytes;
-  const int workers = g_num_sms;
-  const bool use_sk = want_sk && !batch_invariant() && ws_ptr && ws_bytes >= ws_need && p.KB >= 8 && (p.T % g_num_sms) != 0 &&
-                      (long)p.T * p.KB >= g_num_sms;
+  const bool use_sk = want_sk && !batch_invariant() && ws_ptr && ws_bytes >= ws_need && p.KB >= 8 && (p.T % sms) != 0 &&
+                      (long)p.T * p.KB >= sms;
   if (use_sk) {
-    p.G = g_num_sms;
+    p.G = sms;
     const int waves = p.T / p.G;
     p.T_dp = (waves >= 2) ? (waves - 1) * p.G : 0;
     p.U_sk = (long)(p.T - p.T_dp) * p.KB;
     p.sflags = reinterpret_cast<int*>(ws_ptr);
     p.ws = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ws_ptr) + kFlagBytes);
   } else {
-    p.G = workers < p.T ? workers : p.T;
+    p.G = sms < p.T ? sms : p.T;
     p.T_dp = p.T;
     p.U_sk = 0;
   }
@@ -914,8 +906,7 @@ static int launch(const idiff_gemm_args* a, cudaStream_t stream, bool want_sk) {
                                           C::SMEM_BYTES));
     attr_set = true;
   }
-  IDIFF_CHECK_CUDA(launch_pdl(gemm2_kernel<BN, MODE, EPI, LNR>, dim3(p.G), dim3(THREADS), C::SMEM_BYTES, stream, tmA, tmB, tmO, tmR, p));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(idiff::launch(gemm2_kernel<BN, MODE, EPI, LNR>, dim3(p.G), dim3(THREADS), C::SMEM_BYTES, stream, tmA, tmB, tmO, tmR, p));
   return 0;
 }
 
@@ -942,12 +933,7 @@ static int count_m_tiles(const idiff_gemm_args* a) {
 // fixed_bn: 0 = choose the tile width, at most max_bn
 static Plan plan_gemm(const idiff_gemm_args* a, int fixed_bn, int max_bn = 256) {
   const char* force = getenv("IDIFF_GEMM_PLAN");  // "bn,sk" overrides the model (tests, tuning); bn 0 = keep
-  if (g_num_sms == 0) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 132;
-  }
-  const int sms = g_num_sms;
+  const int sms = idiff::num_sms();
   const int KB = (a->K + BK - 1) / BK;
   const int m_tiles = count_m_tiles(a);
   const int cands[4] = {256, 192, 160, 128};

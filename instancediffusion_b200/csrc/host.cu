@@ -1,7 +1,6 @@
 // Error text + TMA descriptor encoding (driver entry point resolved at run time, so the
 // library links against cudart only and loads on a GPU-less box).
 #include "host.cuh"
-#include <stdlib.h>
 
 #include <mutex>
 #include <string.h>
@@ -75,14 +74,6 @@ int encode_tmap_f16_sw(CUtensorMap* map, const void* base, int rank, const uint6
                      box[0], rank > 1 ? box[1] : 0, rank > 2 ? box[2] : 0, rank > 3 ? box[3] : 0);
   }
   return 0;
-}
-
-bool pdl_enabled() {
-  static const bool on = []() {
-    const char* e = getenv("IDIFF_PDL");
-    return e && e[0] == '1';  // opt-in: measured neutral on the UNet forward (17.44 vs 17.43 ms)
-  }();
-  return on;
 }
 
 int num_sms() {

@@ -1,10 +1,12 @@
-// Host-side helpers shared by the launchers: error reporting and TMA tensor-map encoding.
+// Host-side helpers shared by the launchers: error reporting, kernel launch, grid sizing and TMA tensor-map encoding.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdint.h>
 #include <stdio.h>
+
+#include <utility>
 
 #ifndef IDIFF_STORAGE_BF16
 #define IDIFF_STORAGE_BF16 0  // see common.cuh: 16-bit storage type of this build
@@ -35,16 +37,14 @@ int encode_tmap_f16(CUtensorMap* map, const void* base, int rank, const uint64_t
 int encode_tmap_f16_sw(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
                        const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes);
 
-// Launch with programmatic stream serialization ("programmatic dependent launch"): the kernel may
-// become resident while its predecessor in the stream is still running; every kernel of this library
-// calls pdl_wait() (common.cuh) before it touches global memory, so only launch latency and prologues
-// (barrier init, descriptor prefetch) overlap.  About 500 dependent launches make one
-// UNet forward.  Opt-in with IDIFF_PDL=1: measured neutral inside the CUDA graph (the big kernels fill
-// the register file, so a successor cannot become resident before they exit); plain stream order is
-// the default.
-bool pdl_enabled();
 // multiprocessor count of the current device (queried once; grid sizes of the bandwidth-bound kernels)
 int num_sms();
+// Grid of a grid-stride kernel over `total` items: one item per thread, at most `ctas_per_sm` CTAs per SM, at least one CTA.
+inline int grid_for(long total, int threads, int ctas_per_sm) {
+  const long g = (total + threads - 1) / threads;
+  const long cap = (long)num_sms() * ctas_per_sm;
+  return g < 1 ? 1 : g > cap ? (int)cap : (int)g;
+}
 // idiff_set_batch_invariant: reduction geometry must not depend on the batch, M or num_sms()
 bool batch_invariant();
 // Pixel chunks per image of a batch-invariant GroupNorm / ScaleU reduction over hw x channels: about 8K elements
@@ -55,48 +55,31 @@ inline int invariant_chunks(int hw, int channels, int max_chunks) {
   const long c = ((long)hw * channels + 8191) / 8192;
   return c < 1 ? 1 : c > max_chunks ? max_chunks : (int)c;
 }
+// Launch `kernel` as thread-block clusters of `cluster_x` CTAs along x (1 = no cluster attribute).  Returns the
+// launch's error, or else cudaGetLastError(), so IDIFF_CHECK_CUDA(launch_cluster(...)) checks the whole launch.
 template <typename... KArgs, typename... Args>
-cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                       Args&&... args) {
+cudaError_t launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                           int cluster_x, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cluster_x;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  cfg.numAttrs = cluster_x > 1 ? 1 : 0;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-// same, launched as thread-block clusters of `cluster_x` CTAs along x (1 = no cluster attribute)
+// launch_cluster without a cluster attribute
 template <typename... KArgs, typename... Args>
-cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                               int cluster_x, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int n = 0;
-  if (cluster_x > 1) {
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = cluster_x;
-    attr[n].val.clusterDim.y = 1;
-    attr[n].val.clusterDim.z = 1;
-    ++n;
-  }
-  if (pdl_enabled()) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = n;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+cudaError_t launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
+  return launch_cluster(kernel, grid, block, smem, stream, 1, std::forward<Args>(args)...);
 }
 
 }  // namespace idiff

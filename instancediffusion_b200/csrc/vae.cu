@@ -17,8 +17,6 @@ namespace idiff {
 __global__ void __launch_bounds__(256)
 vae_latent_in_kernel(const float* __restrict__ z, const float* __restrict__ w, const float* __restrict__ bias,
                      float inv_scale, uint4* __restrict__ out, int B, int C, int HW) {
-  pdl_launch_dependents();
-  pdl_wait();
   __shared__ float sw[64], sb[8];
   if (threadIdx.x < C * C) sw[threadIdx.x] = w[threadIdx.x];
   if (threadIdx.x < C) sb[threadIdx.x] = bias[threadIdx.x];
@@ -52,8 +50,6 @@ vae_latent_in_kernel(const float* __restrict__ z, const float* __restrict__ w, c
 // one CTA per row; the row lives in shared memory as fp32 between the passes
 __global__ void __launch_bounds__(256)
 softmax_rows_kernel(h16* __restrict__ x, int n, long ld) {
-  pdl_launch_dependents();
-  pdl_wait();
   extern __shared__ float srow[];
   __shared__ float red[8];
   h16* row = x + (long)blockIdx.x * ld;
@@ -133,8 +129,6 @@ template <typename T, bool VEC>
 __global__ void __launch_bounds__(256)
 decode_to_image_kernel(const T* __restrict__ x, uint8_t* __restrict__ out, int B, long HW) {
   constexpr int C = 3;
-  pdl_launch_dependents();
-  pdl_wait();
   const long groups = (HW + 3) / 4;
   const long total = (long)B * groups;
   for (long g = (long)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (long)gridDim.x * blockDim.x) {
@@ -174,8 +168,6 @@ encode_posterior_kernel(const float* __restrict__ h, const float* __restrict__ w
                         float scale, const unsigned long long* __restrict__ seeds, const int* __restrict__ index,
                         float* __restrict__ z, int B, long hw) {
   constexpr int ZC = 4, MC = 2 * ZC;
-  pdl_launch_dependents();
-  pdl_wait();
   __shared__ float sw[MC * MC], sb[MC];
   if (threadIdx.x < MC * MC) sw[threadIdx.x] = w[threadIdx.x];
   if (threadIdx.x < MC) sb[threadIdx.x] = bias[threadIdx.x];
@@ -232,11 +224,11 @@ extern "C" int idiff_vae_latent_in(const float* z, const float* w, const float* 
   using namespace idiff;
   IDIFF_REQUIRE(z && w && bias && out, "idiff_vae_latent_in: null pointer argument");
   IDIFF_REQUIRE(channels >= 1 && channels <= 8, "idiff_vae_latent_in: 1..8 latent channels supported (got %d)", channels);
+  IDIFF_REQUIRE(batch > 0 && hw > 0, "idiff_vae_latent_in: bad shape (batch %d, hw %d)", batch, hw);
   const long total = (long)batch * hw;
-  const int blocks = (int)((total + 255) / 256 < num_sms() * 8 ? (total + 255) / 256 : num_sms() * 8);
-  IDIFF_CHECK_CUDA(launch_pdl(vae_latent_in_kernel, dim3(blocks), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), z, w,
-                              bias, inv_scale, reinterpret_cast<uint4*>(out), batch, channels, hw));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  const int blocks = grid_for(total, 256, 8);
+  IDIFF_CHECK_CUDA(launch(vae_latent_in_kernel, dim3(blocks), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream), z, w,
+                          bias, inv_scale, reinterpret_cast<uint4*>(out), batch, channels, hw));
   return 0;
 }
 
@@ -251,9 +243,8 @@ extern "C" int idiff_softmax_rows(void* x, int rows, int n, long ld, void* strea
     IDIFF_CHECK_CUDA(cudaFuncSetAttribute(softmax_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     attr_set = true;
   }
-  IDIFF_CHECK_CUDA(launch_pdl(softmax_rows_kernel, dim3(rows), dim3(256), smem, reinterpret_cast<cudaStream_t>(stream),
-                              reinterpret_cast<h16*>(x), n, ld));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  IDIFF_CHECK_CUDA(launch(softmax_rows_kernel, dim3(rows), dim3(256), smem, reinterpret_cast<cudaStream_t>(stream),
+                          reinterpret_cast<h16*>(x), n, ld));
   return 0;
 }
 
@@ -263,19 +254,18 @@ extern "C" int idiff_decode_to_image(const void* x, int x_fp32, void* out, int b
   const bool vec = hw % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & (x_fp32 ? 15 : 7)) == 0 &&
                    (reinterpret_cast<uintptr_t>(out) & 3) == 0;
   const long total = (long)batch * ((hw + 3) / 4);
-  const int blocks = (int)((total + 255) / 256 < num_sms() * 16 ? (total + 255) / 256 : num_sms() * 16);
+  const int blocks = grid_for(total, 256, 16);
   const cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   uint8_t* o = reinterpret_cast<uint8_t*>(out);
   if (x_fp32) {
     const float* xf = reinterpret_cast<const float*>(x);
-    IDIFF_CHECK_CUDA(vec ? launch_pdl(decode_to_image_kernel<float, true>, dim3(blocks), dim3(256), 0, s, xf, o, batch, hw)
-                         : launch_pdl(decode_to_image_kernel<float, false>, dim3(blocks), dim3(256), 0, s, xf, o, batch, hw));
+    IDIFF_CHECK_CUDA(vec ? launch(decode_to_image_kernel<float, true>, dim3(blocks), dim3(256), 0, s, xf, o, batch, hw)
+                         : launch(decode_to_image_kernel<float, false>, dim3(blocks), dim3(256), 0, s, xf, o, batch, hw));
   } else {
     const h16* xh = reinterpret_cast<const h16*>(x);
-    IDIFF_CHECK_CUDA(vec ? launch_pdl(decode_to_image_kernel<h16, true>, dim3(blocks), dim3(256), 0, s, xh, o, batch, hw)
-                         : launch_pdl(decode_to_image_kernel<h16, false>, dim3(blocks), dim3(256), 0, s, xh, o, batch, hw));
+    IDIFF_CHECK_CUDA(vec ? launch(decode_to_image_kernel<h16, true>, dim3(blocks), dim3(256), 0, s, xh, o, batch, hw)
+                         : launch(decode_to_image_kernel<h16, false>, dim3(blocks), dim3(256), 0, s, xh, o, batch, hw));
   }
-  IDIFF_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -286,9 +276,8 @@ extern "C" int idiff_encode_posterior(const float* h, const float* w, const floa
   IDIFF_REQUIRE(h && w && bias && seeds && index && z, "idiff_encode_posterior: null pointer argument");
   IDIFF_REQUIRE(batch > 0 && hw > 0, "idiff_encode_posterior: bad shape (batch %d, hw %ld)", batch, hw);
   const long total = (long)batch * 4 * ((hw + 3) / 4);
-  const int blocks = (int)((total + 255) / 256 < num_sms() * 16 ? (total + 255) / 256 : num_sms() * 16);
-  IDIFF_CHECK_CUDA(launch_pdl(encode_posterior_kernel, dim3(blocks), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-                              h, w, bias, scale, seeds, index, z, batch, hw));
-  IDIFF_CHECK_CUDA(cudaGetLastError());
+  const int blocks = grid_for(total, 256, 16);
+  IDIFF_CHECK_CUDA(launch(encode_posterior_kernel, dim3(blocks), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
+                          h, w, bias, scale, seeds, index, z, batch, hw));
   return 0;
 }
