@@ -274,6 +274,23 @@ int idiff_noise_latent(const float* x_init, long n_init, float sqrt_a, float sqr
 int idiff_encode_posterior(const float* h, const float* w, const float* bias, float scale,
                            const unsigned long long* seeds, const int* index, float* z, int batch, long hw,
                            void* stream);
+/* ---------------------------------------------------------------------------------------------
+ * idiff_inpaint_blend: the inpainting blend of a request's `count` trajectories before an evaluation (plms.py:99-103,
+ * ddim.py:94-97) with a seeded noise, all fp32 except keep, out of place, for every trajectory k and element i of the
+ * (batch, channels, hw) latent, b = i / (channels*hw), p = i % hw:
+ *   outs[k][i] = keep[(b % keep_batch)*hw + p] ? sqrt_a*x0[i % (x0_batch*channels*hw)] + sqrt_1m_a*z_i : xs[k][i]
+ * xs_dev / outs_dev are device arrays of `count` pointers; xs may repeat a pointer, the outputs must be distinct from
+ * each other and from every input.  x0 is (x0_batch, channels, hw) and keep uint8 (keep_batch, hw), nonzero = keep;
+ * x0_batch and keep_batch are 1 or batch.  sqrt_a / sqrt_1m_a are the diffusion's fp32 sqrt_alphas_cumprod[t] and
+ * sqrt_one_minus_alphas_cumprod[t]; the two products and the sum are each rounded to fp32, so a kept element is exactly
+ * q_sample(x0, t) with noise z.  z_i is a standard normal that depends on (seed, t, i) alone: Philox4x32-10 with key
+ * (seed & 0xffffffff, seed >> 32) and counter (c & 0xffffffff, c >> 32, t, 3), c = i/4, then Box-Muller on the four
+ * words exactly as in idiff_ddim_update.  Counter word 3 is 0 for the DDIM eta noise, 1 for the image-to-image start
+ * noise, 2 for the encoder posterior and 3 here: one seed keys all four streams.
+ * ------------------------------------------------------------------------------------------- */
+int idiff_inpaint_blend(const float* const* xs_dev, float* const* outs_dev, int count, const float* x0,
+                        const void* keep, int batch, int x0_batch, int keep_batch, int channels, long hw,
+                        float sqrt_a, float sqrt_1m_a, unsigned long long seed, int t, void* stream);
 /* out = mean over `count` latents given as an array of device pointers (plms_instance.py:135) */
 int idiff_latent_mean(const float* const* xs_dev, int count, float* out, long n, void* stream);
 

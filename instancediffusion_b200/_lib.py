@@ -81,6 +81,7 @@ SIGNATURES = {
     "idiff_ddim_update": (_i, [_vp, _vp, _vp, _f, _f, _f, _f, C.c_uint64, _i, _vp, _vp, _l, _vp]),
     "idiff_dpmpp2m_update": (_i, [_vp, _vp, _vp, _f, _vp, _f, _f, _f, _f, _f, _f, _vp, _vp, _l, _vp]),
     "idiff_noise_latent": (_i, [_vp, _l, _f, _f, C.c_uint64, _vp, _l, _vp]),
+    "idiff_inpaint_blend": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _i, _i, _l, _f, _f, C.c_uint64, _i, _vp]),
     "idiff_latent_mean": (_i, [_vp, _i, _vp, _l, _vp]),
     "idiff_conv_in_select": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "idiff_encode_image_in": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),

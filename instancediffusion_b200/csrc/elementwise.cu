@@ -252,6 +252,51 @@ __global__ void noise_latent_kernel(const float* __restrict__ x_init, long n_ini
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// inpainting blend of a request's trajectories before an evaluation (plms.py:99-103, ddim.py:94-97) with a seeded z
+// ---------------------------------------------------------------------------------------------
+// One thread per group of four elements 4c .. 4c+3 of the (B, C, H, W) latent: Philox4x32-10 at counter (c lo, c hi, t,
+// 3) and key (seed lo, seed hi), Box-Muller as in ddim_update_kernel, drawn only when the group has a kept element (z
+// depends on (seed, t, i) alone, so skipping it changes nothing).  Counter word 3 = 3 keeps the stream disjoint from the
+// DDIM eta (0), start (1) and encoder posterior (2) noise.  A kept element is q_sample(x0, t) = sqrt_a * x0 +
+// sqrt_1m_a * z, each product and the sum rounded on their own as torch computes it; the thread writes its group to
+// every trajectory's output.  x0 is broadcast over the batch (element i reads i % n_x0), keep over the channels (pixel
+// b * hw + p reads (b * hw + p) % n_keep).  xs may repeat a pointer (the trajectories of a Multi-instance run share
+// their start latent), so the latent pointers are not restrict.
+__global__ void inpaint_blend_kernel(const float* const* __restrict__ xs, float* const* __restrict__ outs, int count,
+                                     const float* __restrict__ x0, long n_x0, const uint8_t* __restrict__ keep,
+                                     long n_keep, long chw, long hw, float sqrt_a, float sqrt_1m_a, uint2 key,
+                                     uint32_t t, long n) {
+  const long groups = (n + 3) / 4;
+  for (long c = (long)blockIdx.x * blockDim.x + threadIdx.x; c < groups; c += (long)gridDim.x * blockDim.x) {
+    bool kept[4];
+    bool any = false;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long i = 4 * c + j;
+      kept[j] = i < n && keep[((i / chw) * hw + i % hw) % n_keep] != 0;
+      any |= kept[j];
+    }
+    float z[4] = {0.f, 0.f, 0.f, 0.f};
+    if (any) {
+      const uint4 v = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)((unsigned long long)c >> 32), t, 3u), key);
+      box_muller(v.x, v.y, z[0], z[1]);
+      box_muller(v.z, v.w, z[2], z[3]);
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long i = 4 * c + j;
+      if (i >= n) break;
+      if (kept[j]) {
+        const float q = __fadd_rn(__fmul_rn(sqrt_a, x0[i % n_x0]), __fmul_rn(sqrt_1m_a, z[j]));
+        for (int k = 0; k < count; ++k) outs[k][i] = q;
+      } else {
+        for (int k = 0; k < count; ++k) outs[k][i] = xs[k][i];
+      }
+    }
+  }
+}
+
 __global__ void latent_mean_kernel(const float* const* __restrict__ xs, int count, float* __restrict__ out,
                                    long n) {
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
@@ -514,6 +559,24 @@ extern "C" int idiff_noise_latent(const float* x_init, long n_init, float sqrt_a
   IDIFF_CHECK_CUDA(launch(noise_latent_kernel, dim3(grid_for(groups, 256, 16)), dim3(256), 0,
                           reinterpret_cast<cudaStream_t>(stream), x_init, n_init, sqrt_a, sqrt_1m_a, key, x_out,
                           n));
+  return 0;
+}
+
+extern "C" int idiff_inpaint_blend(const float* const* xs_dev, float* const* outs_dev, int count, const float* x0,
+                                   const void* keep, int batch, int x0_batch, int keep_batch, int channels, long hw,
+                                   float sqrt_a, float sqrt_1m_a, unsigned long long seed, int t, void* stream) {
+  IDIFF_REQUIRE(xs_dev && outs_dev && x0 && keep, "idiff_inpaint_blend: null pointer argument");
+  IDIFF_REQUIRE(count > 0 && batch > 0 && channels > 0 && hw > 0 && t >= 0 && (x0_batch == 1 || x0_batch == batch) &&
+                    (keep_batch == 1 || keep_batch == batch),
+                "idiff_inpaint_blend: bad arguments (count %d, batch %d, x0 batch %d, keep batch %d, channels %d, "
+                "hw %ld, t %d)", count, batch, x0_batch, keep_batch, channels, hw, t);
+  const long chw = (long)channels * hw, n = batch * chw;
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  const long groups = (n + 3) / 4;
+  IDIFF_CHECK_CUDA(launch(inpaint_blend_kernel, dim3(grid_for(groups, 256, 16)), dim3(256), 0,
+                          reinterpret_cast<cudaStream_t>(stream), xs_dev, outs_dev, count, x0, x0_batch * chw,
+                          reinterpret_cast<const uint8_t*>(keep), keep_batch * hw, chw, hw, sqrt_a, sqrt_1m_a, key,
+                          (uint32_t)t, n));
   return 0;
 }
 

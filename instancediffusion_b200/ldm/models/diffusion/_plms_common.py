@@ -349,7 +349,15 @@ class SamplingRun:
     the alpha schedule `alphas` (None: none) and, for image-to-image, `x_init`.  A driver calls `start`, then per
     evaluation `begin`, one evaluation of `trajs` and `advance` with its eps, until `i` reaches `steps`; `finish`
     returns the latent.  After the predictor of a first PLMS step `pending` is set and the next evaluation is the
-    corrector's, at t_next of the same step."""
+    corrector's, at t_next of the same step.
+
+    `keep` (uint8 (1 or B, H, W), nonzero = keep; set before `start`, needs x_init) makes the run an inpainting run:
+    before each evaluation `begin` replaces the kept cells of every trajectory by q_sample(x_init, t) whose noise is
+    keyed by (`base.seed`, t) (`ops.inpaint_blend`), so the request's latent depends on its own seed alone.  This is
+    not the `blend` argument of `begin` twice: that one is the drop-in samplers' mask / x0, which draws its noise from
+    torch's global generator in `diffusion.q_sample` exactly as the reference does, so a drop-in run reproduces the
+    reference's draws; `keep` serves the request drivers, whose requests must be reproducible from their seed however
+    they are batched."""
 
     def __init__(self, base: PLMSBase, inputs: List[dict], shape, plan: RequestPlan, guidance_scale: float,
                  alphas: Optional[Sequence[float]], x_init: Optional[torch.Tensor] = None):
@@ -357,6 +365,8 @@ class SamplingRun:
         self.gs = float(guidance_scale)
         self.alphas = alphas
         self.x_init = x_init
+        self.keep: Optional[torch.Tensor] = None
+        self.blend_x0 = None   # x_init as the blend reads it (fp32, contiguous, on the device), set by `start`
         self.time_range = np.flip(base.ddim_timesteps)
         self.steps = len(self.time_range)
         self.trajs: List[Trajectory] = []
@@ -378,6 +388,24 @@ class SamplingRun:
             for inp in self.ins:
                 inp["x"] = img
         self.trajs = [Trajectory(inp) for inp in self.ins[:self.plan.trajectories]]
+        if self.keep is not None:
+            if self.x_init is None:
+                raise ValueError("an inpainting run (keep mask) needs x_init, the kept region's latent")
+            dev = self.base.device
+            self.keep = self.keep.to(device=dev, dtype=torch.uint8).contiguous()
+            self.blend_x0 = self.x_init.to(device=dev, dtype=torch.float32).contiguous()
+            d = self.base.diffusion  # the fp32 scalars q_sample reads, fetched once for the run
+            self.blend_coefs = (d.sqrt_alphas_cumprod.cpu(), d.sqrt_one_minus_alphas_cumprod.cpu())
+
+    def inpaint(self, t: int):
+        """The seeded inpainting blend at timestep t: every trajectory's latent becomes a new tensor whose kept cells
+        are q_sample(x_init, t) (`ops.inpaint_blend`, one launch for all trajectories)."""
+        xs = [tr.input["x"].float().contiguous() for tr in self.trajs]
+        outs = [torch.empty_like(xs[0]) for _ in xs]
+        a = (float(self.blend_coefs[0][t]), float(self.blend_coefs[1][t]))
+        ops.inpaint_blend(xs, outs, self.blend_x0, self.keep, a, self.base.seed, t)
+        for tr, out in zip(self.trajs, outs):
+            tr.input["x"] = out
 
     def merge(self):
         """Multi-instance merge: the global trajectory continues from the mean of the n+1 latents
@@ -391,14 +419,17 @@ class SamplingRun:
 
     def begin(self, blend: Optional[Tuple[torch.Tensor, torch.Tensor]] = None):
         """Before an evaluation: the merge due before step i, the timesteps of step i and, with `blend` = (mask, x0),
-        the inpainting blend x = q_sample(x0, t) * mask + (1 - mask) * x -- unless the evaluation is the corrector's
-        of a first PLMS step (the predictor left the inputs at t_next)."""
+        the inpainting blend x = q_sample(x0, t) * mask + (1 - mask) * x, or with the run's `keep` mask the seeded
+        blend (`inpaint`) -- unless the evaluation is the corrector's of a first PLMS step (the predictor left the
+        inputs at t_next)."""
         if self.pending is None:
             if self.plan.merge_step == self.i:
                 self.merge()
             ts, self.ts_next = self.base._timesteps(self.plan.images, self.i, self.time_range)
             for tr in self.trajs:
                 tr.input["timesteps"] = ts
+            if self.keep is not None:
+                self.inpaint(int(self.time_range[self.i]))
             if blend is not None:
                 mask, x0 = blend
                 assert x0 is not None

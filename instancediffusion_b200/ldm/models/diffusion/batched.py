@@ -17,14 +17,21 @@ with `output="image"` gets the image of its latent instead: the drivers decode t
 together in batched first-stage forwards (`decode_latents`), eagerly and apart from the UNet's caches and graphs.  A
 request may also start from an image (`init_image`, uint8): the drivers encode the images of the requests that start
 together in batched first-stage forwards (`encode_images`), eagerly, before those requests' start latents, and the
-request then runs as if it had been given x_init = autoencoder.encode_images(init_image, seed=its seed).
+request then runs as if it had been given x_init = autoencoder.encode_images(init_image, seed=its seed).  An
+image-to-image request may also repaint part of its image (`repaint_mask`, inpainting): before every evaluation the
+latent cells outside the mask are replaced by x_init noised to the step's timestep, with a noise keyed by the request's
+seed and the timestep (`SamplingRun.inpaint`), so everything outside the mask stays the source's; an image output of
+an `init_image` request takes the source's pixels outside the mask (`paste_back`).
 
 Contract: each returned latent equals, within floating-point tolerance, what `PLMSSampler.sample()` (input dict,
 mis = 0), `PLMSSamplerInst.sample()` (input list [global, instance_1 .. instance_n]), `DDIMSampler.sample(eta=,
 seed=)` or `DPMSolverSampler.sample()` returns for that request alone on the model in the state it had when
 `sample_requests` was called; for an `init_image` request, what the same request with x_init =
-`AutoencoderKL.encode_images(init_image, seed=seed)` returns (bit for bit in batch-invariant mode).
-Afterwards the model's fuser scale and first-conv swap are what a sequential run of the same requests would leave.
+`AutoencoderKL.encode_images(init_image, seed=seed)` returns (bit for bit in batch-invariant mode); for an inpainting
+request (`repaint_mask`), what its sampler's `sample_loop(mask=keep, x0=x_init, x_init=x_init, ...)` returns alone
+with `diffusion.q_sample` drawing its noise from the seeded blend stream (`ops.inpaint_blend`) instead of torch's
+global generator.  Afterwards the model's fuser scale and first-conv swap are what a sequential run of the same
+requests would leave.
 """
 from __future__ import annotations
 
@@ -46,8 +53,9 @@ class Request:
     """One sampling request.  `input`: the dict `PLMSSampler.sample` takes, or the list [global, inst_1 .. inst_n]
     of `PLMSSamplerInst.sample`; `shape`: (B, 4, H, W) of its latent (may be omitted when input x is given);
     `mis`: the Multi-instance fraction (list inputs only).  `S`: the request's step count; `sample_requests` takes it
-    from the call (S, if given, must equal it), `SamplingEngine` requires it.  `mask` / `x0` (inpainting) are not
-    supported and raise.  `sampler`: a name of `SAMPLERS`: "plms", "ddim" (`DDIMSampler.sample`: input dict only)
+    from the call (S, if given, must equal it), `SamplingEngine` requires it.  `mask` / `x0` (the reference's inpainting,
+    whose noise comes from torch's global generator and so depends on what ran before) are not supported and raise:
+    inpainting requests use `repaint_mask`.  `sampler`: a name of `SAMPLERS`: "plms", "ddim" (`DDIMSampler.sample`: input dict only)
     with its `eta` and `seed` (None at eta > 0: one draw from torch's default CPU generator when `sample_requests`
     starts or at `submit`, in request order), or "dpmpp_2m" (`DPMSolverSampler.sample`: input dict only, eta = 0).  `x_init`: a latent of
     shape (1 or B, C, H, W) to start image-to-image sampling from, which runs the last int(N * strength) of the N schedule steps (the samplers' `x_init` / `strength`); the start noise is
@@ -56,7 +64,19 @@ class Request:
     `init_image`: instead of x_init, uint8 RGB images (1 or B, 8H, 8W, 3) on any device, which the driver's
     `autoencoder` encodes with the request's seed (`AutoencoderKL.encode_images(init_image, seed=seed)`) into the x_init
     the request starts from; one image on a B > 1 request is encoded once and broadcast.  The request is not modified:
-    the latent stays with the driver."""
+    the latent stays with the driver.
+
+    `repaint_mask`: inpainting, a bool or uint8 tensor (1 or B, 8H, 8W) at pixel resolution on any device, nonzero =
+    regenerate this pixel; it needs x_init or init_image, the source of the kept region.  A latent cell (y, x) is
+    repainted if any pixel of [8y, 8y+8) x [8x, 8x+8) is; before every evaluation (not the corrector's of a first PLMS
+    step) every other cell of every trajectory is set to q_sample(x_init, t) at the step's timestep t, its noise keyed
+    by (seed, t), as `PLMSBase.sample_loop(mask=, x0=x_init)` blends (plms.py:99-103).  `strength` keeps its meaning:
+    1 is classic inpainting from x_init noised at the first timestep, below 1 the masked region is also repainted
+    SDEdit-style from the noised source.  Every sampler kind takes it, and Multi-instance requests blend every
+    trajectory before the merge with the same source latent (as `sample_loop(mis=, mask=, x0=)`; the drop-in
+    `PLMSSamplerInst.sample` ignores mask / x0, as the reference's does).  An `output="image"` request started from
+    `init_image` returns the source's bytes wherever the mask is zero (`paste_back`); one started from x_init has no
+    source pixels and returns the decoded image as it is."""
     input: Union[dict, List[dict]]
     uc: Optional[torch.Tensor] = None
     guidance_scale: float = 1.0
@@ -73,6 +93,7 @@ class Request:
     strength: float = 1.0
     output: str = "latent"
     init_image: Optional[torch.Tensor] = None
+    repaint_mask: Optional[torch.Tensor] = None
 
 
 SAMPLERS = {kind.sampler: kind for kind in (PLMSBase, DDIMBase, DPMSolverBase)}
@@ -97,7 +118,8 @@ def schedule_steps(S: int, ddpm_timesteps: int = 1000) -> int:
 
 def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_timesteps: int = 1000) -> List[RequestPlan]:
     """Validate the requests of one `sample_requests` call and describe them for the planner.  All must share the
-    step count S, the latent height x width and the context length; mask / x0 inpainting is not supported.
+    step count S, the latent height x width and the context length; mask / x0 inpainting is not supported (inpainting
+    requests give `repaint_mask`).
     A Multi-instance request merges before step int(schedule_steps(S) * mis), as PLMSSamplerInst does (an
     image-to-image one only if that step lies after its start step k0, `PLMSBase.mis_merge_step`)."""
     if not 0 < int(S) <= int(ddpm_timesteps):
@@ -112,7 +134,8 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
         if req.S is not None and int(req.S) != int(S):
             raise ValueError(f"request {j}: S={req.S} differs from the call's S={S}")
         if req.mask is not None or req.x0 is not None:
-            raise ValueError(f"request {j}: mask / x0 inpainting is not supported by sample_requests")
+            raise ValueError(f"request {j}: mask / x0 inpainting is not supported by the request drivers; use "
+                             "repaint_mask with x_init or init_image")
         multi = isinstance(req.input, (list, tuple))
         kind = SAMPLERS.get(req.sampler)
         if kind is None:
@@ -171,6 +194,17 @@ def check_requests(requests: Sequence[Request], S: int, max_batch: int, ddpm_tim
             if im.dim() != 4 or im.shape[0] not in (1, shape[0]) or tuple(im.shape[1:]) != want:
                 raise ValueError(f"request {j}: init_image of shape {tuple(im.shape)} does not fit the latent {shape} "
                                  f"(want (1 or B, {want[0]}, {want[1]}, 3): 8x the latent, RGB)")
+        if req.repaint_mask is not None:
+            m = req.repaint_mask
+            if not isinstance(m, torch.Tensor) or m.dtype not in (torch.bool, torch.uint8):
+                raise ValueError(f"request {j}: repaint_mask must be a bool or uint8 tensor, got "
+                                 f"{getattr(m, 'dtype', type(m).__name__)}")
+            want = (8 * shape[2], 8 * shape[3])
+            if m.dim() != 3 or m.shape[0] not in (1, shape[0]) or tuple(m.shape[1:]) != want:
+                raise ValueError(f"request {j}: repaint_mask of shape {tuple(m.shape)} does not fit the latent {shape} "
+                                 f"(want (1 or B, {want[0]}, {want[1]}): 8x the latent)")
+            if req.x_init is None and req.init_image is None:
+                raise ValueError(f"request {j}: repaint_mask needs x_init or init_image (the source of the kept region)")
         img2img = req.x_init is not None or req.init_image is not None
         plans.append(RequestPlan.of(len(ins), req.mis if multi else None, steps, k0, img2img, shape[0],
                                     req.uc is not None and req.guidance_scale != 1))
@@ -214,6 +248,8 @@ class _RequestState(SamplingRun):
     def start(self):
         if self.req.init_image is not None and self.x_init is None:
             raise RuntimeError("an init_image request starts after `encode_init_images`")
+        if self.req.repaint_mask is not None:
+            self.keep = keep_mask(self.req.repaint_mask.to(self.base.device))
         super().start()
 
     def images(self) -> int:
@@ -312,6 +348,24 @@ class _RequestState(SamplingRun):
                     setattr(model, k, saved[k])
                 else:
                     delattr(model, k)
+
+
+def keep_mask(repaint_mask: torch.Tensor) -> torch.Tensor:
+    """The latent keep mask of a pixel repaint mask (Bm, 8H, 8W): uint8 (Bm, H, W), 1 where no pixel of the cell's 8x8
+    block is to be repainted."""
+    bm, h8, w8 = repaint_mask.shape
+    rep = (repaint_mask != 0).view(bm, h8 // 8, 8, w8 // 8, 8).any(4).any(2)
+    return (~rep).to(torch.uint8)
+
+
+def paste_back(req: Request, image: torch.Tensor) -> torch.Tensor:
+    """The image of a finished request: for an inpainting request started from `init_image`, the decoded `image`
+    (B, 8H, 8W, 3) inside its repaint mask and the source's bytes outside it, out[b, y, x] = repaint[b % Bm, y, x] ?
+    image[b, y, x] : init_image[b % Bi, y, x]; any other request's image as it is."""
+    if req.repaint_mask is None or req.init_image is None:
+        return image
+    rep = req.repaint_mask.to(image.device) != 0
+    return torch.where(rep[..., None], image, req.init_image.to(image.device))
 
 
 def check_decode(requests: Sequence[Request], autoencoder, max_decode_batch: int, max_encode_batch: int = 8) -> None:
@@ -433,5 +487,5 @@ def sample_requests(model, diffusion, requests: Sequence[Union[Request, Dict]], 
     images = [j for j, r in enumerate(reqs) if r.output == "image"]
     if images:
         for j, img in zip(images, decode_latents(autoencoder, [latents[j] for j in images], max_decode_batch)):
-            latents[j] = img
+            latents[j] = paste_back(reqs[j], img)
     return latents

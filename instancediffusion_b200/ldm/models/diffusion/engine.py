@@ -14,6 +14,9 @@ instead of its latent: the image requests that finish in a tick are decoded toge
 request with an `init_image` starts from that image: the `init_image` requests admitted in a tick are encoded together
 in that tick, before their start latents and forwards, at most `max_encode_batch` images per encoder forward
 (`batched.encode_images`), eagerly, outside the UNet's graphs, each with its own seed (drawn at `submit` when None).
+An inpainting request (`repaint_mask`) blends its kept cells into its trajectories in `begin`, eagerly, before the
+tick's forwards, so the blend stays outside the captured graphs and adds none; its image output takes the source's
+pixels outside the mask (`batched.paste_back`).
 
 A tick gives every live trajectory exactly one UNet evaluation: the one at t of its current step or, for a request
 in the Euler predictor of its first PLMS step, the corrector's evaluation at t_next (so the corrector rides in the
@@ -38,7 +41,8 @@ Contract: each returned latent equals, within floating-point tolerance, what the
 `PLMSSampler.sample()` / `PLMSSamplerInst.sample()` / `DDIMSampler.sample(eta=, seed=)` / `DPMSolverSampler.sample()`
 returns when it runs alone on the model in the state it had at `submit`, whatever else is live and whenever the
 request arrived; an `init_image` request's equals that of the same request with x_init =
-`AutoencoderKL.encode_images(init_image, seed=seed)`.
+`AutoencoderKL.encode_images(init_image, seed=seed)`; an inpainting request's equals its sampler's
+`sample_loop(mask=keep, x0=x_init, ...)` with the seeded blend noise (batched.py).
 """
 from __future__ import annotations
 
@@ -47,7 +51,8 @@ from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 
-from .batched import Request, RequestPlan, _RequestState, check_decode, check_requests, decode_latents, plan_chunks
+from .batched import (Request, RequestPlan, _RequestState, check_decode, check_requests, decode_latents, paste_back,
+                      plan_chunks)
 
 
 def pick_bucket(images: int, unit: int, buckets: Optional[Sequence[int]]) -> Optional[int]:
@@ -180,11 +185,11 @@ class SamplingEngine:
         if finished:
             keep = [i for st in list(self._live.values()) + [st for _, st in self._queue] for i in st.inputs()]
             self.model.drop_hoisted([i for st in finished for i in st.inputs()], keep)
-        images = [t for t, st in zip(done, finished) if st.req.output == "image"]
+        images = [(t, st.req) for t, st in zip(done, finished) if st.req.output == "image"]
         if images:
-            for t, img in zip(images, decode_latents(self.autoencoder, [done[t] for t in images],
-                                                     self.max_decode_batch)):
-                done[t] = img
+            for (t, req), img in zip(images, decode_latents(self.autoencoder, [done[t] for t, _ in images],
+                                                            self.max_decode_batch)):
+                done[t] = paste_back(req, img)
         return done
 
     def _run(self, states, forwards, scales, flags):

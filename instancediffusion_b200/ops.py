@@ -559,6 +559,59 @@ def noise_latent(x_init: torch.Tensor, a: float, seed: int, out: torch.Tensor) -
     return out
 
 
+def inpaint_blend(xs, outs, x0: torch.Tensor, keep: torch.Tensor, a: Tuple[float, float], seed: int, t: int):
+    """The inpainting blend of one request's trajectories (include/idiff_b200.h idiff_inpaint_blend), out of place:
+    outs[k] = where(keep, sqrt_a * x0 + sqrt_1m_a * z, xs[k]) for every trajectory k, in one launch.  xs / outs: lists
+    of fp32 contiguous (B, C, H, W) tensors (xs may repeat a tensor; the outputs are distinct and none of them is an
+    input); x0 fp32 (1 or B, C, H, W), broadcast over the batch; keep uint8 (1 or B, H, W), nonzero = keep, broadcast
+    over the channels.  a = (sqrt_a, sqrt_1m_a): the diffusion's fp32 sqrt_alphas_cumprod[t] and
+    sqrt_one_minus_alphas_cumprod[t], each in [0, 1], passed as they are so a kept element is exactly q_sample(x0, t)
+    with noise z.  z is a function of (seed, t, element) only; seed an integer in [0, 2^64), t >= 0."""
+    lib = _lib.load()
+    xs, outs = list(xs), list(outs)
+    if not xs or len(xs) != len(outs):
+        raise _lib.IdiffError(f"inpaint_blend: {len(xs)} inputs and {len(outs)} outputs (want the same, > 0)")
+    shape = tuple(xs[0].shape)
+    if len(shape) != 4 or 0 in shape:
+        raise _lib.IdiffError(f"inpaint_blend: latent shape {shape} is not a non-empty (B, C, H, W)")
+    B, Cc, H, W = shape
+    for name, ts in (("xs", xs), ("outs", outs)):
+        for t_ in ts:
+            _req(t_, torch.float32, name)
+            if tuple(t_.shape) != shape or not t_.is_contiguous() or t_.device != xs[0].device:
+                raise _lib.IdiffError(f"inpaint_blend: every tensor of {name} must be a contiguous {shape} tensor on "
+                                      f"{xs[0].device}")
+    out_ptrs = [o.data_ptr() for o in outs]
+    if len(set(out_ptrs)) != len(out_ptrs) or set(out_ptrs) & {x.data_ptr() for x in xs}:
+        raise _lib.IdiffError("inpaint_blend: the outputs must be distinct tensors, none of them an input")
+    _req(x0, torch.float32, "x0")
+    _req(keep, torch.uint8, "keep")
+    for name, t_, want in (("x0", x0, (Cc, H, W)), ("keep", keep, (H, W))):
+        if (t_.dim() != len(want) + 1 or t_.shape[0] not in (1, B) or tuple(t_.shape[1:]) != want
+                or not t_.is_contiguous() or t_.device != xs[0].device):
+            raise _lib.IdiffError(f"inpaint_blend: {name} of shape {tuple(t_.shape)} is not a contiguous "
+                                  f"(1 or {B}, {', '.join(map(str, want))}) tensor on {xs[0].device}")
+    sqrt_a, sqrt_1m_a = (float(v) for v in a)
+    if not (0.0 <= sqrt_a <= 1.0 and 0.0 <= sqrt_1m_a <= 1.0):
+        raise _lib.IdiffError(f"inpaint_blend: a={a} outside [0, 1]")
+    seed, t = int(seed), int(t)
+    if not 0 <= seed < 1 << 64:
+        raise _lib.IdiffError(f"inpaint_blend: seed {seed} outside [0, 2^64)")
+    if not 0 <= t < 1 << 31:
+        raise _lib.IdiffError(f"inpaint_blend: t={t} outside [0, 2^31)")
+    # pinned and non-blocking: a copy from pageable memory would wait for the stream's queued work (the previous step's
+    # forwards) on every call, once per request and step
+    ptrs = torch.tensor([x.data_ptr() for x in xs] + out_ptrs, dtype=torch.int64,
+                        pin_memory=True).to(x0.device, non_blocking=True)
+    n = xs[0].numel()
+    check(_launch("inpaint_blend", 0.0, 4.0 * (len(xs) * 2 * n + x0.numel()) + keep.numel(),
+                  lambda: lib.idiff_inpaint_blend(ptrs.data_ptr(), ptrs.data_ptr() + 8 * len(xs), len(xs),
+                                                  x0.data_ptr(), keep.data_ptr(), B, x0.shape[0], keep.shape[0], Cc,
+                                                  H * W, sqrt_a, sqrt_1m_a, seed, t, _stream())),
+          "idiff_inpaint_blend")
+    return outs
+
+
 def latent_mean(xs, out: torch.Tensor) -> torch.Tensor:
     lib = _lib.load()
     ptrs = torch.tensor([t.data_ptr() for t in xs], dtype=torch.int64).to(out.device)
