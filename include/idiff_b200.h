@@ -222,14 +222,26 @@ int idiff_plms_update(const float* x, const float* e_c, const float* e_u, float 
                       float c2, float c3, float a_t, float a_prev, float sqrt_one_minus_at,
                       float* e_out, float* x_out, long n, void* stream);
 /* ---------------------------------------------------------------------------------------------
+ * Seeded noise.  idiff_ddim_update, idiff_noise_latent, idiff_encode_posterior and idiff_inpaint_blend draw their
+ * standard normals z_i from counter-based streams, so z_i is a pure function of (seed, stream, word 2, i): it does not
+ * depend on the launch shape, the batch or the tensor length beyond i.  Elements 4c..4c+3 come from Philox4x32-10
+ * with key (seed & 0xffffffff, seed >> 32) and counter (c & 0xffffffff, c >> 32, word 2, stream), whose four words
+ * v0..v3 give z by Box-Muller on (v0, v1) and (v2, v3): u = (v + 0.5)*2^-32, r = sqrt(-2 ln u_a),
+ * z = r cos(2 pi u_b), then r sin(2 pi u_b).  Counter word 3 names the stream, so one seed keys all of them and no
+ * two share a counter:
+ *   0  DDIM eta noise                 (idiff_ddim_update)
+ *   1  image-to-image start noise     (idiff_noise_latent)
+ *   2  encoder posterior              (idiff_encode_posterior)
+ *   3  inpainting blend               (idiff_inpaint_blend)
+ * Saved seeds reproduce their images only while these numbers stay as they are; a new stream takes the next one.
+ * ------------------------------------------------------------------------------------------- */
+/* ---------------------------------------------------------------------------------------------
  * idiff_ddim_update: fused DDIM step (ddim.py:116-131), all fp32, n elements:
  *   e      = e_u + gs*(e_c - e_u)         (CFG; e_u may be NULL -> e = e_c)
  *   pred0  = (x - sqrt(1-a_t)*e) / sqrt(a_t)
  *   x_out  = sqrt(a_prev)*pred0 + sqrt(max(1-a_prev-sigma^2, 0))*e + sigma*z_i
- * z_i (drawn only for sigma > 0) is a standard normal that depends on (seed, index, i) alone: Philox4x32-10 with key
- * (seed & 0xffffffff, seed >> 32) and counter (c & 0xffffffff, c >> 32, index, 0), c = i/4, whose four words v0..v3
- * give elements 4c..4c+3 by Box-Muller on (v0, v1) and (v2, v3): u = (v + 0.5)*2^-32, r = sqrt(-2 ln u_a),
- * z = r cos(2 pi u_b), then r sin(2 pi u_b).  With x = 0, e_c = 0, e_u = NULL and sigma = 1, x_out is z.
+ * z_i (drawn only for sigma > 0) is seeded noise (see "Seeded noise") of stream 0 with word 2 = index.  With x = 0,
+ * e_c = 0, e_u = NULL and sigma = 1, x_out is z.
  * e_out (may be NULL) receives the post-CFG e.
  * ------------------------------------------------------------------------------------------- */
 int idiff_ddim_update(const float* x, const float* e_c, const float* e_u, float gs, float a_t, float a_prev,
@@ -252,10 +264,8 @@ int idiff_dpmpp2m_update(const float* x, const float* e_c, const float* e_u, flo
 /* ---------------------------------------------------------------------------------------------
  * idiff_noise_latent: start latent of image-to-image sampling (SDEdit), all fp32, n elements:
  *   x_out[i] = sqrt_a*x_init[i % n_init] + sqrt_1m_a*z_i          (n % n_init == 0: x_init broadcast over the batch)
- * z_i is a standard normal that depends on (seed, i) alone: Philox4x32-10 with key (seed & 0xffffffff, seed >> 32)
- * and counter (c & 0xffffffff, c >> 32, 0, 1), c = i/4, then Box-Muller on the four words exactly as in
- * idiff_ddim_update.  Counter word 3 is 1 here and 0 there, so the two streams never share a counter and one seed can
- * key both.  With x_init = 0, sqrt_a = 0 and sqrt_1m_a = 1, x_out is z.
+ * z_i is seeded noise (see "Seeded noise") of stream 1 with word 2 = 0.  With x_init = 0, sqrt_a = 0 and
+ * sqrt_1m_a = 1, x_out is z.
  * ------------------------------------------------------------------------------------------- */
 int idiff_noise_latent(const float* x_init, long n_init, float sqrt_a, float sqrt_1m_a, unsigned long long seed,
                        float* x_out, long n, void* stream);
@@ -265,11 +275,9 @@ int idiff_noise_latent(const float* x_init, long n_init, float sqrt_a, float sqr
  *   mean   = m[0:4],  logvar = clamp(m[4:8], -30, 20),  std = exp(0.5 * logvar)
  *   z      = (mean + std * eps) * scale            (each product and sum rounded on its own)
  * h (batch, 8, hw) NCHW, the encoder's conv_out; w [8][8], bias [8]; z (batch, 4, hw).  eps of element e = c*hw + p of
- * image b is a standard normal that depends on (seeds[b], index[b], e) alone: Philox4x32-10 with key
- * (seed & 0xffffffff, seed >> 32) and counter (c' & 0xffffffff, c' >> 32, index[b], 2), c' = e/4, word e % 4 after
- * Box-Muller exactly as in idiff_ddim_update.  seeds (uint64) and index (int32, the image's position in its request)
- * are per-image arrays in device memory, so one launch serves the images of many requests.  Counter word 3 is 0 for
- * the DDIM eta noise, 1 for the image-to-image start noise and 2 here: one seed keys all three streams.
+ * image b is z_e of seeded noise (see "Seeded noise") of stream 2 with seed seeds[b] and word 2 = index[b].  seeds
+ * (uint64) and index (int32, the image's position in its request) are per-image arrays in device memory, so one
+ * launch serves the images of many requests.
  * ------------------------------------------------------------------------------------------- */
 int idiff_encode_posterior(const float* h, const float* w, const float* bias, float scale,
                            const unsigned long long* seeds, const int* index, float* z, int batch, long hw,
@@ -283,10 +291,7 @@ int idiff_encode_posterior(const float* h, const float* w, const float* bias, fl
  * each other and from every input.  x0 is (x0_batch, channels, hw) and keep uint8 (keep_batch, hw), nonzero = keep;
  * x0_batch and keep_batch are 1 or batch.  sqrt_a / sqrt_1m_a are the diffusion's fp32 sqrt_alphas_cumprod[t] and
  * sqrt_one_minus_alphas_cumprod[t]; the two products and the sum are each rounded to fp32, so a kept element is exactly
- * q_sample(x0, t) with noise z.  z_i is a standard normal that depends on (seed, t, i) alone: Philox4x32-10 with key
- * (seed & 0xffffffff, seed >> 32) and counter (c & 0xffffffff, c >> 32, t, 3), c = i/4, then Box-Muller on the four
- * words exactly as in idiff_ddim_update.  Counter word 3 is 0 for the DDIM eta noise, 1 for the image-to-image start
- * noise, 2 for the encoder posterior and 3 here: one seed keys all four streams.
+ * q_sample(x0, t) with noise z.  z_i is seeded noise (see "Seeded noise") of stream 3 with word 2 = t.
  * ------------------------------------------------------------------------------------------- */
 int idiff_inpaint_blend(const float* const* xs_dev, float* const* outs_dev, int count, const float* x0,
                         const void* keep, int batch, int x0_batch, int keep_batch, int channels, long hw,

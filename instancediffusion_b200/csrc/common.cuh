@@ -263,4 +263,23 @@ IDIFF_DEVICE void box_muller(uint32_t a, uint32_t b, float& z0, float& z1) {
   z1 = r * s;
 }
 
+// Seeded noise streams (include/idiff_b200.h, "Seeded noise").  Counter word 3 names the stream, so one seed keys all
+// of them without overlap.  Saved seeds and the goldens under tests/golden/ depend on these values: never renumber one,
+// only append.
+enum NoiseStream : uint32_t { kNoiseDdimEta = 0, kNoiseStart = 1, kNoisePosterior = 2, kNoiseInpaint = 3 };
+
+// Philox key of a 64-bit seed: (seed lo, seed hi).
+__host__ __device__ __forceinline__ uint2 philox_key(unsigned long long seed) {
+  return make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+}
+
+// The four normals of element group `group` (elements 4 group .. 4 group + 3) of a stream: Philox4x32-10 at counter
+// (group lo, group hi, word2, stream), then Box-Muller on (v0, v1) and (v2, v3).
+IDIFF_DEVICE void normals4(uint2 key, long group, uint32_t word2, NoiseStream stream, float (&z)[4]) {
+  const uint4 v =
+      philox4x32_10(make_uint4((uint32_t)group, (uint32_t)((unsigned long long)group >> 32), word2, stream), key);
+  box_muller(v.x, v.y, z[0], z[1]);
+  box_muller(v.z, v.w, z[2], z[3]);
+}
+
 }  // namespace idiff

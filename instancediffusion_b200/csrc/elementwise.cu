@@ -172,9 +172,8 @@ __global__ void plms_update_kernel(const float* __restrict__ x, const float* __r
 // ---------------------------------------------------------------------------------------------
 // fused DDIM update (ddim.py:116-131) with its eta noise drawn in place
 // ---------------------------------------------------------------------------------------------
-// One thread per group of four elements 4c .. 4c+3: Philox4x32-10 at counter (c lo, c hi, index, 0) and key
-// (seed lo, seed hi) gives four words, Box-Muller on (v0, v1) and (v2, v3) their four normals.  So z_i depends on
-// (seed, index, i) only, not on the launch shape, the tensor length beyond i or the batch.  sigma == 0 draws nothing.
+// One thread per group of four elements 4c .. 4c+3, noise from stream kNoiseDdimEta with word 2 = index (normals4), so
+// z_i depends on (seed, index, i) alone.  sigma == 0 draws nothing.
 __global__ void ddim_update_kernel(const float* __restrict__ x, const float* __restrict__ e_c,
                                    const float* __restrict__ e_u, float gs, float sqrt_at, float sqrt_1m_at,
                                    float sqrt_aprev, float sqrt_dir, float sigma, uint2 key, uint32_t index,
@@ -182,11 +181,7 @@ __global__ void ddim_update_kernel(const float* __restrict__ x, const float* __r
   const long groups = (n + 3) / 4;
   for (long c = (long)blockIdx.x * blockDim.x + threadIdx.x; c < groups; c += (long)gridDim.x * blockDim.x) {
     float z[4] = {0.f, 0.f, 0.f, 0.f};
-    if (sigma > 0.f) {
-      const uint4 v = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)((unsigned long long)c >> 32), index, 0u), key);
-      box_muller(v.x, v.y, z[0], z[1]);
-      box_muller(v.z, v.w, z[2], z[3]);
-    }
+    if (sigma > 0.f) normals4(key, c, index, kNoiseDdimEta, z);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const long i = 4 * c + j;
@@ -232,17 +227,14 @@ __global__ void dpmpp2m_update_kernel(const float* __restrict__ x, const float* 
 // ---------------------------------------------------------------------------------------------
 // image-to-image start latent: x_init noised to the start timestep (q_sample with a seeded z)
 // ---------------------------------------------------------------------------------------------
-// One thread per group of four elements 4c .. 4c+3: Philox4x32-10 at counter (c lo, c hi, 0, 1) and key (seed lo,
-// seed hi), Box-Muller as in ddim_update_kernel.  Counter word 3 = 1 keeps the stream disjoint from the DDIM eta
-// noise (word 3 = 0), so one seed can key both.  x_init is broadcast over the batch: element i reads i % n_init.
+// One thread per group of four elements 4c .. 4c+3, noise from stream kNoiseStart with word 2 = 0 (normals4).  x_init
+// is broadcast over the batch: element i reads i % n_init.
 __global__ void noise_latent_kernel(const float* __restrict__ x_init, long n_init, float sqrt_a, float sqrt_1m_a,
                                     uint2 key, float* __restrict__ x_out, long n) {
   const long groups = (n + 3) / 4;
   for (long c = (long)blockIdx.x * blockDim.x + threadIdx.x; c < groups; c += (long)gridDim.x * blockDim.x) {
     float z[4];
-    const uint4 v = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)((unsigned long long)c >> 32), 0u, 1u), key);
-    box_muller(v.x, v.y, z[0], z[1]);
-    box_muller(v.z, v.w, z[2], z[3]);
+    normals4(key, c, 0u, kNoiseStart, z);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const long i = 4 * c + j;
@@ -255,14 +247,13 @@ __global__ void noise_latent_kernel(const float* __restrict__ x_init, long n_ini
 // ---------------------------------------------------------------------------------------------
 // inpainting blend of a request's trajectories before an evaluation (plms.py:99-103, ddim.py:94-97) with a seeded z
 // ---------------------------------------------------------------------------------------------
-// One thread per group of four elements 4c .. 4c+3 of the (B, C, H, W) latent: Philox4x32-10 at counter (c lo, c hi, t,
-// 3) and key (seed lo, seed hi), Box-Muller as in ddim_update_kernel, drawn only when the group has a kept element (z
-// depends on (seed, t, i) alone, so skipping it changes nothing).  Counter word 3 = 3 keeps the stream disjoint from the
-// DDIM eta (0), start (1) and encoder posterior (2) noise.  A kept element is q_sample(x0, t) = sqrt_a * x0 +
-// sqrt_1m_a * z, each product and the sum rounded on their own as torch computes it; the thread writes its group to
-// every trajectory's output.  x0 is broadcast over the batch (element i reads i % n_x0), keep over the channels (pixel
-// b * hw + p reads (b * hw + p) % n_keep).  xs may repeat a pointer (the trajectories of a Multi-instance run share
-// their start latent), so the latent pointers are not restrict.
+// One thread per group of four elements 4c .. 4c+3 of the (B, C, H, W) latent, noise from stream kNoiseInpaint with
+// word 2 = t (normals4), drawn only when the group has a kept element (z depends on (seed, t, i) alone, so skipping it
+// changes nothing).  A kept element is q_sample(x0, t) = sqrt_a * x0 + sqrt_1m_a * z, each product and the sum rounded
+// on their own as torch computes it; the thread writes its group to every trajectory's output.  x0 is broadcast over
+// the batch (element i reads i % n_x0), keep over the channels (pixel b * hw + p reads (b * hw + p) % n_keep).  xs may
+// repeat a pointer (the trajectories of a Multi-instance run share their start latent), so the latent pointers are not
+// restrict.
 __global__ void inpaint_blend_kernel(const float* const* __restrict__ xs, float* const* __restrict__ outs, int count,
                                      const float* __restrict__ x0, long n_x0, const uint8_t* __restrict__ keep,
                                      long n_keep, long chw, long hw, float sqrt_a, float sqrt_1m_a, uint2 key,
@@ -278,11 +269,7 @@ __global__ void inpaint_blend_kernel(const float* const* __restrict__ xs, float*
       any |= kept[j];
     }
     float z[4] = {0.f, 0.f, 0.f, 0.f};
-    if (any) {
-      const uint4 v = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)((unsigned long long)c >> 32), t, 3u), key);
-      box_muller(v.x, v.y, z[0], z[1]);
-      box_muller(v.z, v.w, z[2], z[3]);
-    }
+    if (any) normals4(key, c, t, kNoiseInpaint, z);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const long i = 4 * c + j;
@@ -533,11 +520,10 @@ extern "C" int idiff_ddim_update(const float* x, const float* e_c, const float* 
   // the fp32 coefficients of ddim.py:118-129: sqrt(1 - a_prev - sigma^2) clamped at 0 (eta <= 1 keeps it >= 0 up to
   // rounding)
   const float sqrt_dir = sqrtf(fmaxf(1.0f - a_prev - sigma * sigma, 0.0f));
-  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   const long groups = (n + 3) / 4;
   IDIFF_CHECK_CUDA(launch(ddim_update_kernel, dim3(grid_for(groups, 256, 16)), dim3(256), 0,
                           reinterpret_cast<cudaStream_t>(stream), x, e_c, e_u, gs, sqrtf(a_t), sqrtf(1.0f - a_t),
-                          sqrtf(a_prev), sqrt_dir, sigma, key, (uint32_t)index, e_out, x_out, n));
+                          sqrtf(a_prev), sqrt_dir, sigma, philox_key(seed), (uint32_t)index, e_out, x_out, n));
   return 0;
 }
 
@@ -554,11 +540,10 @@ extern "C" int idiff_dpmpp2m_update(const float* x, const float* e_c, const floa
 extern "C" int idiff_noise_latent(const float* x_init, long n_init, float sqrt_a, float sqrt_1m_a,
                                   unsigned long long seed, float* x_out, long n, void* stream) {
   IDIFF_REQUIRE(x_init && x_out && n > 0 && n_init > 0 && n % n_init == 0, "idiff_noise_latent: bad arguments");
-  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   const long groups = (n + 3) / 4;
   IDIFF_CHECK_CUDA(launch(noise_latent_kernel, dim3(grid_for(groups, 256, 16)), dim3(256), 0,
-                          reinterpret_cast<cudaStream_t>(stream), x_init, n_init, sqrt_a, sqrt_1m_a, key, x_out,
-                          n));
+                          reinterpret_cast<cudaStream_t>(stream), x_init, n_init, sqrt_a, sqrt_1m_a, philox_key(seed),
+                          x_out, n));
   return 0;
 }
 
@@ -571,12 +556,11 @@ extern "C" int idiff_inpaint_blend(const float* const* xs_dev, float* const* out
                 "idiff_inpaint_blend: bad arguments (count %d, batch %d, x0 batch %d, keep batch %d, channels %d, "
                 "hw %ld, t %d)", count, batch, x0_batch, keep_batch, channels, hw, t);
   const long chw = (long)channels * hw, n = batch * chw;
-  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   const long groups = (n + 3) / 4;
   IDIFF_CHECK_CUDA(launch(inpaint_blend_kernel, dim3(grid_for(groups, 256, 16)), dim3(256), 0,
                           reinterpret_cast<cudaStream_t>(stream), xs_dev, outs_dev, count, x0, x0_batch * chw,
-                          reinterpret_cast<const uint8_t*>(keep), keep_batch * hw, chw, hw, sqrt_a, sqrt_1m_a, key,
-                          (uint32_t)t, n));
+                          reinterpret_cast<const uint8_t*>(keep), keep_batch * hw, chw, hw, sqrt_a, sqrt_1m_a,
+                          philox_key(seed), (uint32_t)t, n));
   return 0;
 }
 

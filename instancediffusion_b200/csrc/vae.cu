@@ -160,9 +160,9 @@ decode_to_image_kernel(const T* __restrict__ x, uint8_t* __restrict__ out, int B
 
 // One thread per latent channel c of a group of four pixels p0 .. p0+3 of one image: the eight conv_out planes of those
 // pixels in, the mean and logvar rows of quant_conv (1x1, 8 -> 8, fp32 FMAs in input-channel order), the posterior
-// sample out.  The noise of element e = c*hw + p of image b is word e % 4 of Philox4x32-10 at counter (e/4 lo, e/4 hi,
-// index[b], 2) and key (seed lo, seed hi) after Box-Muller, so it depends on (seed, index, e) alone; with hw % 4 == 0
-// one Philox call serves the thread's four pixels.
+// sample out.  The noise of element e = c*hw + p of image b is normal e % 4 of group e / 4 of stream kNoisePosterior
+// with key seeds[b] and word 2 = index[b] (normals4), so it depends on (seed, index, e) alone; with hw % 4 == 0 one draw
+// serves the thread's four pixels.
 __global__ void __launch_bounds__(256)
 encode_posterior_kernel(const float* __restrict__ h, const float* __restrict__ w, const float* __restrict__ bias,
                         float scale, const unsigned long long* __restrict__ seeds, const int* __restrict__ index,
@@ -192,8 +192,7 @@ encode_posterior_kernel(const float* __restrict__ h, const float* __restrict__ w
         logvar[j] = fmaf(sw[(c + ZC) * MC + k], v, logvar[j]);
       }
     }
-    const unsigned long long seed = seeds[b];
-    const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+    const uint2 key = philox_key(seeds[b]);
     const uint32_t idx = (uint32_t)index[b];
     float* zb = z + ((long)b * ZC + c) * hw + p0;
     long cached = -1;
@@ -204,9 +203,7 @@ encode_posterior_kernel(const float* __restrict__ h, const float* __restrict__ w
       const long e = c * hw + p0 + j;
       if ((e >> 2) != cached) {
         cached = e >> 2;
-        const uint4 v = philox4x32_10(make_uint4((uint32_t)cached, (uint32_t)((unsigned long long)cached >> 32), idx, 2u), key);
-        box_muller(v.x, v.y, eps4[0], eps4[1]);
-        box_muller(v.z, v.w, eps4[2], eps4[3]);
+        normals4(key, cached, idx, kNoisePosterior, eps4);
       }
       const int q = (int)(e & 3);  // selected, not indexed, so eps4 stays in registers
       const float eps = q == 0 ? eps4[0] : q == 1 ? eps4[1] : q == 2 ? eps4[2] : eps4[3];

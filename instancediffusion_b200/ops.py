@@ -154,6 +154,14 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
+def _seed(seed, caller: str = "") -> int:
+    """seed as an int in [0, 2^64), the kernels' uint64 key, else IdiffError prefixed with `caller`."""
+    seed = int(seed)
+    if not 0 <= seed < 1 << 64:
+        raise _lib.IdiffError((f"{caller}: " if caller else "") + f"seed {seed} outside [0, 2^64)")
+    return seed
+
+
 def _req(t: torch.Tensor, dtype, name: str) -> None:
     if not t.is_cuda:
         raise _lib.IdiffError(f"{name} must be a CUDA tensor (no CPU fallback exists)")
@@ -507,9 +515,7 @@ def ddim_update(x: torch.Tensor, e_c: torch.Tensor, e_u: Optional[torch.Tensor],
             _req(t, torch.float32, name)
             if t.numel() != x.numel() or not t.is_contiguous():
                 raise _lib.IdiffError(f"ddim_update: {name} must be contiguous with {x.numel()} elements")
-    seed = int(seed)
-    if not 0 <= seed < 1 << 64:
-        raise _lib.IdiffError(f"ddim_update: seed {seed} outside [0, 2^64)")
+    seed = _seed(seed, "ddim_update")
     check(lib.idiff_ddim_update(x.data_ptr(), e_c.data_ptr(), _ptr(e_u), float(gs), float(a_t), float(a_prev),
                                 float(sigma), seed, int(index), _ptr(e_out), x_out.data_ptr(), x.numel(), _stream()),
           "idiff_ddim_update")
@@ -551,9 +557,7 @@ def noise_latent(x_init: torch.Tensor, a: float, seed: int, out: torch.Tensor) -
     a = float(a)
     if not 0.0 <= a <= 1.0:
         raise _lib.IdiffError(f"noise_latent: a={a} outside [0, 1]")
-    seed = int(seed)
-    if not 0 <= seed < 1 << 64:
-        raise _lib.IdiffError(f"noise_latent: seed {seed} outside [0, 2^64)")
+    seed = _seed(seed, "noise_latent")
     check(lib.idiff_noise_latent(x_init.data_ptr(), x_init.numel(), math.sqrt(a), math.sqrt(1.0 - a), seed,
                                  out.data_ptr(), out.numel(), _stream()), "idiff_noise_latent")
     return out
@@ -594,9 +598,7 @@ def inpaint_blend(xs, outs, x0: torch.Tensor, keep: torch.Tensor, a: Tuple[float
     sqrt_a, sqrt_1m_a = (float(v) for v in a)
     if not (0.0 <= sqrt_a <= 1.0 and 0.0 <= sqrt_1m_a <= 1.0):
         raise _lib.IdiffError(f"inpaint_blend: a={a} outside [0, 1]")
-    seed, t = int(seed), int(t)
-    if not 0 <= seed < 1 << 64:
-        raise _lib.IdiffError(f"inpaint_blend: seed {seed} outside [0, 2^64)")
+    seed, t = _seed(seed, "inpaint_blend"), int(t)
     if not 0 <= t < 1 << 31:
         raise _lib.IdiffError(f"inpaint_blend: t={t} outside [0, 2^31)")
     # pinned and non-blocking: a copy from pageable memory would wait for the stream's queued work (the previous step's
@@ -804,10 +806,7 @@ def decode_to_image(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
 
 def seed_array(seeds, device) -> torch.Tensor:
     """Seeds in [0, 2^64) as the uint64 words the kernels read (an int64 tensor with the same bits) on `device`."""
-    seeds = [int(s) for s in seeds]
-    for s in seeds:
-        if not 0 <= s < 1 << 64:
-            raise _lib.IdiffError(f"seed {s} outside [0, 2^64)")
+    seeds = [_seed(s) for s in seeds]
     words = torch.tensor([s - (1 << 64) if s >= 1 << 63 else s for s in seeds], dtype=torch.int64)
     return words.to(device)
 

@@ -2,10 +2,8 @@
 seeded posterior in torch, and a fake first stage whose `encode_images` is torch-only, for the CPU tests of the request
 drivers' `init_image`.
 
-* `posterior_noise(seed, index, n)`: Philox4x32-10 with key (seed lo, seed hi) and counter (c lo, c hi, index, 2),
-  c = e // 4, then Box-Muller as in cases_ddim.ddim_noise (DDIM: counter word 3 = 0; the start noise of
-  cases_img2img.start_noise: word 3 = 1).
-* `posterior(moments, scale, seeds, index)`: distributions.py:24-36 and autoencoder.py:31 with that noise, float64.
+* `posterior(moments, scale, seeds, index)`: distributions.py:24-36 and autoencoder.py:31 with the posterior stream of
+  cases_noise, float64.
 * `FakeAutoencoder`: `AutoencoderKL.encode_images` over a torch stand-in encoder, plus the fake decoder of
   cases_decode; logs the batch of every encode.
 """
@@ -13,29 +11,13 @@ from __future__ import annotations
 
 from typing import Sequence
 
-import numpy as np
 import torch
 
-import cases_ddim as CD
 import cases_decode as CDec
+import cases_noise as CN
 from instancediffusion_b200.ldm.models.autoencoder import AutoencoderKL, check_images
 
-_LO = np.uint64(0xFFFFFFFF)
 SCALE = 0.18215
-
-
-def posterior_noise(seed: int, index: int, n: int) -> np.ndarray:
-    """eps_0 .. eps_{n-1} of image `index` of a request seeded `seed` (float64)."""
-    seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-    c = np.arange((n + 3) // 4, dtype=np.uint64)
-    v = CD.philox4x32([c & _LO, c >> np.uint64(32), np.full(c.shape, index, np.uint32), np.full(c.shape, 2, np.uint32)],
-                      [np.uint32(seed & 0xFFFFFFFF), np.uint32(seed >> 32)]).astype(np.float64)
-    u = (v + 0.5) * 2.0 ** -32
-    z = np.empty((c.shape[0], 4))
-    for a, b in ((0, 1), (2, 3)):
-        r = np.sqrt(-2.0 * np.log(u[a]))
-        z[:, a], z[:, b] = r * np.cos(2 * np.pi * u[b]), r * np.sin(2 * np.pi * u[b])
-    return z.reshape(-1)[:n]
 
 
 def quant_conv64(h: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
@@ -44,11 +26,11 @@ def quant_conv64(h: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> torch.
 
 
 def posterior(moments: torch.Tensor, scale: float, seeds: Sequence[int], index: Sequence[int]) -> torch.Tensor:
-    """(mean + exp(0.5 clamp(logvar, -30, 20)) * eps) * scale in float64 on the CPU, image b's eps
-    posterior_noise(seeds[b], index[b])."""
+    """(mean + exp(0.5 clamp(logvar, -30, 20)) * eps) * scale in float64 on the CPU, image b's eps the posterior stream
+    at (seeds[b], index[b])."""
     m = moments.detach().double().cpu()
     mean, logvar = m[:, :4], m[:, 4:].clamp(-30.0, 20.0)
-    eps = torch.stack([torch.from_numpy(posterior_noise(s, i, mean[0].numel())).view(mean.shape[1:])
+    eps = torch.stack([torch.from_numpy(CN.normals(s, CN.POSTERIOR, i, mean[0].numel())).view(mean.shape[1:])
                        for s, i in zip(seeds, index)])
     return (mean + torch.exp(0.5 * logvar) * eps) * scale
 

@@ -2,10 +2,8 @@
 in numpy, the start latent in float64 and in torch, and the PLMS / DDIM loops from the start step k0 in torch.
 
 * `start_step(N, strength)`: k0 = N - int(N * strength); n_run = int(N * strength) must be >= 1.
-* `start_noise`: Philox4x32-10 with key (seed lo, seed hi) and counter (c lo, c hi, 0, 1), c = i // 4, then Box-Muller as
-  in cases_ddim.ddim_noise (whose DDIM stream has counter word 3 = 0).
-* `x_start64` / `noise_latent`: sqrt(a) * x_init + sqrt(1 - a) * z in float64, and in torch with ops.noise_latent's
-  arguments (what the CPU tests run instead of the kernel).
+* `x_start64` / `noise_latent`: sqrt(a) * x_init + sqrt(1 - a) * z in float64, z the start-noise stream of
+  cases_noise, and in torch with ops.noise_latent's arguments (what the CPU tests run instead of the kernel).
 * `plms_tail` / `ddim_tail`: the samplers' loops over steps k0 .. N-1 (plms.py:72-167, plms_instance.py:65-212,
   ddim.py:63-131), with the Multi-instance rule of a truncated schedule: trajectories merge before int(N * mis) only if
   that step lies after k0.
@@ -18,8 +16,7 @@ import numpy as np
 import torch
 
 import cases_ddim as CD
-
-_LO = np.uint64(0xFFFFFFFF)
+import cases_noise as CN
 
 
 def start_step(steps: int, strength: float) -> int:
@@ -29,24 +26,10 @@ def start_step(steps: int, strength: float) -> int:
     return steps - n_run
 
 
-def start_noise(seed: int, n: int) -> np.ndarray:
-    """z_0 .. z_{n-1} of idiff_noise_latent for `seed`, float64."""
-    seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-    c = np.arange((n + 3) // 4, dtype=np.uint64)
-    v = CD.philox4x32([c & _LO, c >> np.uint64(32), np.zeros(c.shape, np.uint32), np.ones(c.shape, np.uint32)],
-                      [np.uint32(seed & 0xFFFFFFFF), np.uint32(seed >> 32)]).astype(np.float64)
-    u = (v + 0.5) * 2.0 ** -32
-    z = np.empty((c.shape[0], 4))
-    for a, b in ((0, 1), (2, 3)):
-        r = np.sqrt(-2.0 * np.log(u[a]))
-        z[:, a], z[:, b] = r * np.cos(2 * np.pi * u[b]), r * np.sin(2 * np.pi * u[b])
-    return z.reshape(-1)[:n]
-
-
 def x_start64(x_init: torch.Tensor, a: float, seed: int, shape) -> torch.Tensor:
     """The start latent in float64 (CPU): x_init broadcast to `shape`."""
     n = int(np.prod(shape))
-    z = torch.from_numpy(start_noise(seed, n)).view(tuple(shape))
+    z = torch.from_numpy(CN.normals(seed, CN.START, 0, n)).view(tuple(shape))
     x = x_init.detach().double().cpu().expand(tuple(shape))
     return a ** 0.5 * x + (1 - a) ** 0.5 * z
 
@@ -143,7 +126,7 @@ def plms_tail(eval_fn: Callable, inputs: List[dict], uc, S: int, guidance: float
 
 def ddim_tail(eval_fn: Callable, inp: dict, uc, S: int, guidance: float, x_start: torch.Tensor, k0: int,
               eta: float = 0.0, seed: int = 0, alpha_type=None) -> torch.Tensor:
-    """Steps k0 .. N-1 of DDIM from x_start, the eta noise of step index `index` from cases_ddim.ddim_noise."""
+    """Steps k0 .. N-1 of DDIM from x_start, the eta noise of step index `index` from cases_noise."""
     acp, steps, a, a_prev = _schedule(S)
     _, _, _, sig = CD.ddim_schedule(S, eta, acp)
     time_range = np.flip(steps)
@@ -158,7 +141,7 @@ def ddim_tail(eval_fn: Callable, inp: dict, uc, S: int, guidance: float, x_start
         at, ap, s = float(a[index]), float(a_prev[index]), float(sig[index])
         x = ap ** 0.5 * (inp["x"] - (1. - at) ** 0.5 * e) / at ** 0.5 + max(1. - ap - s * s, 0.) ** 0.5 * e
         if s > 0:
-            z = torch.from_numpy(CD.ddim_noise(seed, index, x.numel())).view_as(x).to(x.device, x.dtype)
+            z = torch.from_numpy(CN.normals(seed, CN.DDIM_ETA, index, x.numel())).view_as(x).to(x.device, x.dtype)
             x = x + s * z
         inp["x"] = x
     return inp["x"]

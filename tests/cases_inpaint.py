@@ -1,12 +1,10 @@
-"""Inpainting requests restated for the tests: the blend's noise stream in numpy, the blend in torch, the seeded
-q_sample the samplers are compared with, the pixel-to-latent mask reduction, and the reference-golden cases.
+"""Inpainting requests restated for the tests: the blend in torch, the seeded q_sample the samplers are compared with,
+the pixel-to-latent mask reduction, and the reference-golden cases.
 
-* `blend_noise(seed, t, n)`: Philox4x32-10 with key (seed lo, seed hi) and counter (c lo, c hi, t, 3), c = i // 4, then
-  Box-Muller as in cases_ddim.ddim_noise (DDIM eta: word 3 = 0, start noise: 1, encoder posterior: 2).
 * `inpaint_blend`: idiff_inpaint_blend in torch (same arguments as ops.inpaint_blend), what the CPU tests run instead of
   the kernel; `inpaint_blend64` the same in float64 for the kernel tests.
-* `seeded_q_sample(diffusion, seed)`: `diffusion.q_sample` with its noise from `blend_noise` at the timestep, the
-  function the samplers' mask / x0 blend is patched with to compare them with inpainting requests.
+* `seeded_q_sample(diffusion, seed)`: `diffusion.q_sample` with its noise from the inpainting stream of cases_noise at
+  the timestep, the function the samplers' mask / x0 blend is patched with to compare them with inpainting requests.
 * `keep_of(repaint)`: a latent cell is kept when no pixel of its 8x8 block is to be repainted.
 * `INPAINT_CASES`: the reference's PLMSSampler / DDIMSampler (eta 0) with mask / x0 on the seeded UNet of
   cases.UNET_CASE; tools/make_golden_inpaint.py writes tests/golden/inpaint.pt.
@@ -16,9 +14,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-import cases_ddim as CD
-
-_LO = np.uint64(0xFFFFFFFF)
+import cases_noise as CN
 
 # name -> spec; the UNet, flavour and 64x64 latent are those of cases.UNET_CASE.  `box` is the repainted pixel box
 # (y0, y1, x0, x1) of the 512x512 image, `src_seed` seeds the source latent x_init, `seed` the blend / start noise.
@@ -28,20 +24,6 @@ INPAINT_CASES = {
     "ddim_S10_b2": dict(sampler="ddim", S=10, n=2, batch=2, seed=72, src_seed=82, input_seed=62, guidance=7.5,
                         alpha_type=[0.8, 0.0, 0.2], box=(203, 461, 37, 300)),  # crosses alpha 0, unaligned box
 }
-
-
-def blend_noise(seed: int, t: int, n: int) -> np.ndarray:
-    """z_0 .. z_{n-1} of idiff_inpaint_blend at (seed, t), float64."""
-    seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-    c = np.arange((n + 3) // 4, dtype=np.uint64)
-    v = CD.philox4x32([c & _LO, c >> np.uint64(32), np.full(c.shape, t, np.uint32), np.full(c.shape, 3, np.uint32)],
-                      [np.uint32(seed & 0xFFFFFFFF), np.uint32(seed >> 32)]).astype(np.float64)
-    u = (v + 0.5) * 2.0 ** -32
-    z = np.empty((c.shape[0], 4))
-    for a, b in ((0, 1), (2, 3)):
-        r = np.sqrt(-2.0 * np.log(u[a]))
-        z[:, a], z[:, b] = r * np.cos(2 * np.pi * u[b]), r * np.sin(2 * np.pi * u[b])
-    return z.reshape(-1)[:n]
 
 
 def keep_of(repaint: torch.Tensor) -> torch.Tensor:
@@ -62,7 +44,7 @@ def box_mask(b: int, size: int, box, dtype=torch.bool) -> torch.Tensor:
 def q_value(x0: torch.Tensor, sqrt_a: float, sqrt_1m_a: float, seed: int, t: int, shape) -> torch.Tensor:
     """sqrt_a * x0 + sqrt_1m_a * z over `shape` (x0 broadcast), in x0's dtype, z rounded to it first."""
     n = int(np.prod(shape))
-    z = torch.from_numpy(blend_noise(seed, t, n)).view(tuple(shape)).to(x0.device, x0.dtype)
+    z = torch.from_numpy(CN.normals(seed, CN.INPAINT, t, n)).view(tuple(shape)).to(x0.device, x0.dtype)
     return sqrt_a * x0.expand(tuple(shape)) + sqrt_1m_a * z
 
 

@@ -1,17 +1,25 @@
 """A fake UNet for the CPU tests of the request schedulers (`sample_requests`, `SamplingEngine`): its eps is a function
-of each image's inputs, fuser scale and first conv, and it logs every forward.  The two sampler kernels are restated in
-torch (`_plms_update`, `_latent_mean`), and `_alone` runs a request through its own sampler on a fresh fake, which is
-what each scheduler's latent is compared with."""
+of each image's inputs, fuser scale and first conv, and it logs every forward.  The two PLMS kernels are restated in
+torch (`_plms_update`, `_latent_mean`), the `torch_kernels` fixture swaps every sampling kernel for its torch
+restatement, and `_alone` runs a request through its own sampler on a fresh fake, which is what each scheduler's latent
+is compared with."""
 import os
 import sys
 from dataclasses import replace
 from functools import partial
 
+import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import cases_ddim as CD  # noqa: E402
+import cases_decode as CDec  # noqa: E402
+import cases_dpm as CPM  # noqa: E402
+import cases_img2img as CI  # noqa: E402
+import cases_inpaint as CP  # noqa: E402
+from instancediffusion_b200 import ops  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion.batched import Request  # noqa: E402
 from instancediffusion_b200.ldm.modules.attention import GatedSelfAttentionDense  # noqa: E402
 from instancediffusion_b200.utils.model import alpha_generator, set_alpha_scale  # noqa: E402
@@ -63,6 +71,25 @@ class FakeUNet(torch.nn.Module):
 
     def trim_hoisted(self):
         pass
+
+
+@pytest.fixture
+def torch_kernels(monkeypatch):
+    """Every sampling kernel of `ops` that has a torch restatement replaced by it.  Returns the number of calls of each
+    by name."""
+    mirrors = dict(plms_update=_plms_update, latent_mean=_latent_mean, ddim_update=CD.ddim_update,
+                   dpmpp2m_update=CPM.dpmpp2m_update, noise_latent=CI.noise_latent, inpaint_blend=CP.inpaint_blend,
+                   decode_to_image=CDec.decode_to_image)
+    calls = dict.fromkeys(mirrors, 0)
+
+    def counted(name, fn):
+        def call(*args, **kw):
+            calls[name] += 1
+            return fn(*args, **kw)
+        return call
+    for name, fn in mirrors.items():
+        monkeypatch.setattr(ops, name, counted(name, fn))
+    return calls
 
 
 AGEN = partial(alpha_generator, type=[0.8, 0.0, 0.2])

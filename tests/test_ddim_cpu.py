@@ -1,8 +1,8 @@
-"""DDIM sampling without a GPU: the numpy mirror of the kernel's Philox4x32-10 noise stream against the Random123 known
-answers, `DDIMSampler.make_schedule` against a float64 restatement of util.py:73-83, the torch restatement of the
-reference's DDIM loop against its latents (tests/golden/ddim.pt), the drop-in path, request validation, and DDIM
-requests mixed with PLMS ones in `sample_requests` / `SamplingEngine` on the fake UNet of fake_unet.py (the kernel
-replaced by its torch restatement with the mirrored noise)."""
+"""DDIM sampling without a GPU: `DDIMSampler.make_schedule` against a float64 restatement of util.py:73-83, the torch
+restatement of the reference's DDIM loop against its latents (tests/golden/ddim.pt), the drop-in path, request
+validation, and DDIM requests mixed with PLMS ones in `sample_requests` / `SamplingEngine` on the fake UNet of
+fake_unet.py (the kernel replaced by its torch restatement with the mirrored noise; the noise stream itself is tested
+in test_noise_streams_cpu.py)."""
 import os
 import subprocess
 import sys
@@ -16,8 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import cases  # noqa: E402
 import cases_ddim as CD  # noqa: E402
-from fake_unet import AGEN, FakeUNet, _alone, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
-from instancediffusion_b200 import ops  # noqa: E402
+from fake_unet import AGEN, FakeUNet, _alone, _fresh, _req, torch_kernels  # noqa: E402,F401
 from instancediffusion_b200.ldm.models.diffusion.batched import (  # noqa: E402
     Request, RequestPlan, _RequestState, check_requests, sample_requests, schedule_steps)
 from instancediffusion_b200.ldm.models.diffusion.ddim import DDIMSampler  # noqa: E402
@@ -32,31 +31,6 @@ ROOT = os.path.dirname(HERE)
 def diffusion():
     from instancediffusion_b200.ldm.models.diffusion.ldm import LatentDiffusion
     return LatentDiffusion(linear_start=0.00085, linear_end=0.012, timesteps=1000)
-
-
-# ------------------------------------------------------------------------------------------------
-# noise stream
-# ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("ctr,key,want", [
-    ((0, 0, 0, 0), (0, 0), (0x6627e8d5, 0xe169c58d, 0xbc57ac4c, 0x9b00dbd8)),
-    ((0xffffffff,) * 4, (0xffffffff,) * 2, (0x408f276d, 0x41c83b0e, 0xa20bc7c6, 0x6d5451fd)),
-    ((0x243f6a88, 0x85a308d3, 0x13198a2e, 0x03707344), (0xa4093822, 0x299f31d0),
-     (0xd16cfe09, 0x94fdcceb, 0x5001e420, 0x24126ea1)),
-])
-def test_philox_known_answers(ctr, key, want):
-    """Random123's known-answer vectors for Philox4x32-10."""
-    got = CD.philox4x32([np.uint32(c) for c in ctr], [np.uint32(k) for k in key])
-    assert [int(v) for v in got.reshape(-1)] == list(want)
-
-
-def test_noise_is_a_function_of_seed_index_and_element():
-    z = CD.ddim_noise(123, 7, 4099)
-    assert np.array_equal(z[:10], CD.ddim_noise(123, 7, 10))       # a prefix does not depend on the length
-    assert not np.array_equal(z[:16], CD.ddim_noise(124, 7, 16))
-    assert not np.array_equal(z[:16], CD.ddim_noise(123, 6, 16))
-    big = CD.ddim_noise(2 ** 40 + 5, 3, 1 << 16)                     # the high seed word enters the key
-    assert not np.array_equal(big[:16], CD.ddim_noise(5, 3, 16))
-    assert abs(big.mean()) < 5 / 256 and abs(big.var() - 1) < 0.02
 
 
 # ------------------------------------------------------------------------------------------------
@@ -198,13 +172,6 @@ def test_unseeded_requests_draw_from_torchs_generator_in_order(diffusion):
 # ------------------------------------------------------------------------------------------------
 # DDIM requests in the batched paths (fake UNet, kernels restated in torch)
 # ------------------------------------------------------------------------------------------------
-@pytest.fixture
-def torch_kernels(monkeypatch):
-    monkeypatch.setattr(ops, "plms_update", _plms_update)
-    monkeypatch.setattr(ops, "latent_mean", _latent_mean)
-    monkeypatch.setattr(ops, "ddim_update", CD.ddim_update)
-
-
 def _ddim(k, S, eta, seed, **kw):
     return replace(_req(k, S, **kw), sampler="ddim", eta=eta, seed=seed)
 

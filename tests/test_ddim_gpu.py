@@ -14,6 +14,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import cases_ddim as CD  # noqa: E402
+import cases_noise as CN  # noqa: E402
 from test_engine_gpu import _drive  # noqa: E402
 from test_requests_gpu import _fresh, _reset, _run_alone  # noqa: E402
 
@@ -100,7 +101,7 @@ def test_noise_matches_the_cpu_mirror(cuda_device):
     n = 1 << 18
     for seed, index in ((0, 0), (123456789, 9), (2 ** 64 - 1, 49)):
         z = _noise(seed, index, n, cuda_device).double().cpu().numpy()
-        want = CD.ddim_noise(seed, index, n)
+        want = CN.normals(seed, CN.DDIM_ETA, index, n)
         err = np.abs(z - want).max()
         print(f"[noise seed={seed} index={index}] max abs err vs mirror {err:.2e}")
         assert err <= 1e-5, err

@@ -11,11 +11,8 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-import cases_ddim as CD  # noqa: E402
 import cases_decode as CDec  # noqa: E402
-import cases_img2img as CI  # noqa: E402
-from fake_unet import FakeUNet, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
-from instancediffusion_b200 import ops  # noqa: E402
+from fake_unet import FakeUNet, _fresh, _req, torch_kernels  # noqa: E402,F401
 from instancediffusion_b200.ldm.models.diffusion.batched import (  # noqa: E402
     RequestPlan, check_requests, decode_latents, sample_requests)
 from instancediffusion_b200.ldm.models.diffusion.engine import SamplingEngine  # noqa: E402
@@ -25,15 +22,6 @@ from instancediffusion_b200.ldm.models.diffusion.engine import SamplingEngine  #
 def diffusion():
     from instancediffusion_b200.ldm.models.diffusion.ldm import LatentDiffusion
     return LatentDiffusion(linear_start=0.00085, linear_end=0.012, timesteps=1000)
-
-
-@pytest.fixture
-def torch_kernels(monkeypatch):
-    monkeypatch.setattr(ops, "plms_update", _plms_update)
-    monkeypatch.setattr(ops, "latent_mean", _latent_mean)
-    monkeypatch.setattr(ops, "ddim_update", CD.ddim_update)
-    monkeypatch.setattr(ops, "noise_latent", CI.noise_latent)
-    monkeypatch.setattr(ops, "decode_to_image", CDec.decode_to_image)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -12,13 +12,11 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-import cases_ddim as CD  # noqa: E402
 import cases_dpm as CP  # noqa: E402
 import cases_img2img as CI  # noqa: E402
-from fake_unet import AGEN, FakeUNet, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
+from fake_unet import AGEN, FakeUNet, _fresh, _req, torch_kernels  # noqa: E402,F401
 from test_img2img_cpu import ALPHA_TYPE, TOL, _eval_fn, _i2i  # noqa: E402
 from test_img2img_cpu import _alone as _alone_other  # noqa: E402
-from instancediffusion_b200 import ops  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion._plms_common import SamplingRun  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion.batched import (  # noqa: E402
     RequestPlan, _RequestState, check_requests, sample_requests, schedule_steps)
@@ -32,21 +30,6 @@ from instancediffusion_b200.utils.model import set_alpha_scale  # noqa: E402
 def diffusion():
     from instancediffusion_b200.ldm.models.diffusion.ldm import LatentDiffusion
     return LatentDiffusion(linear_start=0.00085, linear_end=0.012, timesteps=1000)
-
-
-@pytest.fixture
-def torch_kernels(monkeypatch):
-    calls = {"dpmpp2m_update": 0}
-
-    def dpm(*args):
-        calls["dpmpp2m_update"] += 1
-        return CP.dpmpp2m_update(*args)
-    monkeypatch.setattr(ops, "plms_update", _plms_update)
-    monkeypatch.setattr(ops, "latent_mean", _latent_mean)
-    monkeypatch.setattr(ops, "ddim_update", CD.ddim_update)
-    monkeypatch.setattr(ops, "noise_latent", CI.noise_latent)
-    monkeypatch.setattr(ops, "dpmpp2m_update", dpm)
-    return calls
 
 
 def _dpm(req):

@@ -1,24 +1,17 @@
-"""`init_image` without a GPU: the request validation, the seed resolution order, the posterior noise stream against the
-DDIM and start-noise streams, how the drivers batch the encode, and `init_image` requests against the same requests given
-x_init = encode_images(init_image, seed=seed) in `sample_requests` and `SamplingEngine`, on the fake UNet with a fake
-first stage (tests/cases_encode.py)."""
+"""`init_image` without a GPU: the request validation, the seed resolution order, how the drivers batch the encode, and
+`init_image` requests against the same requests given x_init = encode_images(init_image, seed=seed) in
+`sample_requests` and `SamplingEngine`, on the fake UNet with a fake first stage (tests/cases_encode.py)."""
 import os
 import sys
 from dataclasses import replace
 
-import numpy as np
 import pytest
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-import cases_ddim as CD  # noqa: E402
-import cases_decode as CDec  # noqa: E402
-import cases_dpm as CP  # noqa: E402
 import cases_encode as CE  # noqa: E402
-import cases_img2img as CI  # noqa: E402
-from fake_unet import FakeUNet, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
-from instancediffusion_b200 import ops  # noqa: E402
+from fake_unet import FakeUNet, _fresh, _req, torch_kernels  # noqa: E402,F401
 from instancediffusion_b200.ldm.models.diffusion.batched import (  # noqa: E402
     RequestPlan, check_requests, encode_images, sample_requests)
 from instancediffusion_b200.ldm.models.diffusion.engine import SamplingEngine  # noqa: E402
@@ -28,16 +21,6 @@ from instancediffusion_b200.ldm.models.diffusion.engine import SamplingEngine  #
 def diffusion():
     from instancediffusion_b200.ldm.models.diffusion.ldm import LatentDiffusion
     return LatentDiffusion(linear_start=0.00085, linear_end=0.012, timesteps=1000)
-
-
-@pytest.fixture
-def torch_kernels(monkeypatch):
-    monkeypatch.setattr(ops, "plms_update", _plms_update)
-    monkeypatch.setattr(ops, "latent_mean", _latent_mean)
-    monkeypatch.setattr(ops, "ddim_update", CD.ddim_update)
-    monkeypatch.setattr(ops, "noise_latent", CI.noise_latent)
-    monkeypatch.setattr(ops, "decode_to_image", CDec.decode_to_image)
-    monkeypatch.setattr(ops, "dpmpp2m_update", CP.dpmpp2m_update)
 
 
 def _img(seed, b=1, size=512):
@@ -93,28 +76,8 @@ def test_missing_autoencoder_and_max_encode_batch(diffusion, torch_kernels):
 
 
 # ------------------------------------------------------------------------------------------------
-# the noise stream and the seeds
+# the seeds
 # ------------------------------------------------------------------------------------------------
-def test_posterior_noise_stream():
-    """Counter word 3 = 2: disjoint from the DDIM eta noise (word 3 = 0, word 2 = step index) and the start noise
-    (word 3 = 1) of the same seed; element e is a function of (seed, index, e) alone."""
-    n = 4 * 4096 + 3
-    for seed in (0, 7, 2 ** 63 + 1, 2 ** 64 - 1):
-        post = CE.posterior_noise(seed, 0, n)
-        assert not np.isin(post, CI.start_noise(seed, n)).any()
-        assert not np.isin(post, CD.ddim_noise(seed, 0, n)).any()
-        assert not np.isin(post, CE.posterior_noise(seed, 1, n)).any()  # the next image of the request
-        assert np.array_equal(CE.posterior_noise(seed, 3, 10), CE.posterior_noise(seed, 3, n)[:10])
-        c = np.arange(3, dtype=np.uint64)
-        words = CD.philox4x32([c, np.zeros(3, np.uint32), np.zeros(3, np.uint32), np.full(3, 2, np.uint32)],
-                              [np.uint32(seed & 0xFFFFFFFF), np.uint32(seed >> 32)])
-        u = (words.astype(np.float64) + 0.5) * 2.0 ** -32
-        r = np.sqrt(-2 * np.log(u[0]))
-        assert np.allclose(post[0:12:4], r * np.cos(2 * np.pi * u[1]), rtol=0, atol=1e-12)
-    z = CE.posterior_noise(123, 5, 200000)
-    assert abs(z.mean()) < 0.01 and abs(z.std() - 1) < 0.01
-
-
 def test_encode_images_seed(torch_kernels):
     vae = CE.FakeAutoencoder()
     im = _img(4, b=2, size=64)

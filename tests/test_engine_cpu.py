@@ -9,16 +9,11 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from fake_unet import FakeUNet, _alone, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
-from instancediffusion_b200 import ops  # noqa: E402
+from fake_unet import FakeUNet, _alone, _fresh, _req, torch_kernels  # noqa: E402,F401
 from instancediffusion_b200.ldm.models.diffusion.batched import RequestPlan, schedule_steps  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion.engine import SamplingEngine, pick_bucket, plan_forwards  # noqa: E402
 
-
-@pytest.fixture(autouse=True)
-def torch_kernels(monkeypatch):
-    monkeypatch.setattr(ops, "plms_update", _plms_update)
-    monkeypatch.setattr(ops, "latent_mean", _latent_mean)
+pytestmark = pytest.mark.usefixtures("torch_kernels")
 
 
 @pytest.fixture

@@ -1,4 +1,4 @@
-"""Image-to-image sampling without a GPU: the start step of a strength, validation, the start-noise stream, the three
+"""Image-to-image sampling without a GPU: the start step of a strength, validation, the start latent, the three
 samplers against the torch restatement of their loops from k0 (tests/cases_img2img.py), the unchanged path without
 x_init, the seed draws, and image-to-image requests of several strengths next to plain PLMS / DDIM / Multi-instance
 ones in `sample_requests` and `SamplingEngine`.  The UNet is the fake of fake_unet.py and the kernels are restated in
@@ -7,16 +7,14 @@ import os
 import sys
 from dataclasses import replace
 
-import numpy as np
 import pytest
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-import cases_ddim as CD  # noqa: E402
 import cases_img2img as CI  # noqa: E402
-from fake_unet import FakeUNet, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
-from instancediffusion_b200 import ops  # noqa: E402
+import cases_noise as CN  # noqa: E402
+from fake_unet import FakeUNet, _fresh, _req, torch_kernels  # noqa: E402,F401
 from instancediffusion_b200.ldm.models.diffusion._plms_common import PLMSBase  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion.batched import (  # noqa: E402
     RequestPlan, _RequestState, check_requests, sample_requests, schedule_steps)
@@ -34,20 +32,6 @@ TOL = dict(rtol=1e-5, atol=1e-6)
 def diffusion():
     from instancediffusion_b200.ldm.models.diffusion.ldm import LatentDiffusion
     return LatentDiffusion(linear_start=0.00085, linear_end=0.012, timesteps=1000)
-
-
-@pytest.fixture
-def torch_kernels(monkeypatch):
-    calls = {"latent_mean": 0}
-
-    def mean(xs, out):
-        calls["latent_mean"] += 1
-        return _latent_mean(xs, out)
-    monkeypatch.setattr(ops, "plms_update", _plms_update)
-    monkeypatch.setattr(ops, "latent_mean", mean)
-    monkeypatch.setattr(ops, "ddim_update", CD.ddim_update)
-    monkeypatch.setattr(ops, "noise_latent", CI.noise_latent)
-    return calls
 
 
 def _x_init(seed, b=1, size=64):
@@ -141,16 +125,9 @@ def test_validation_messages(diffusion):
                        10, 32)
 
 
-def test_start_noise_stream():
-    z = CI.start_noise(123, 4099)
-    assert np.array_equal(z[:10], CI.start_noise(123, 10))
-    assert not np.array_equal(z[:16], CI.start_noise(124, 16))
-    assert not np.array_equal(z[:16], CD.ddim_noise(123, 0, 16))  # disjoint from DDIM's eta stream of the same seed
-    big = CI.start_noise(2 ** 64 - 1, 1 << 16)
-    assert not np.array_equal(big[:16], CI.start_noise(2 ** 32 - 1, 16))
-    assert abs(big.mean()) < 5 / 256 and abs(big.var() - 1) < 0.02
+def test_x_start64_noises_x_init_with_the_start_stream():
     x = CI.x_start64(torch.ones((1, 4, 2, 2)), 0.25, 7, (3, 4, 2, 2))
-    want = 0.5 + 0.75 ** 0.5 * torch.from_numpy(CI.start_noise(7, 48)).view(3, 4, 2, 2)
+    want = 0.5 + 0.75 ** 0.5 * torch.from_numpy(CN.normals(7, CN.START, 0, 48)).view(3, 4, 2, 2)
     assert torch.allclose(x, want, rtol=0, atol=1e-15)
 
 

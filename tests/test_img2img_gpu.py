@@ -16,6 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import cases  # noqa: E402
 import cases_img2img as CI  # noqa: E402
+import cases_noise as CN  # noqa: E402
 from test_ddim_gpu import DDIM_LATENT_TOL, _rel, diffusion, unet  # noqa: E402,F401 (module fixtures)
 from test_engine_gpu import _drive  # noqa: E402
 from test_requests_gpu import _fresh, _reset  # noqa: E402
@@ -63,7 +64,7 @@ def test_noise_latent_is_z_at_a_0_and_independent_of_the_build(cuda_device):
             z[dtype] = ops.noise_latent(torch.zeros(n, device=cuda_device), 0.0, 77, torch.empty(n, device=cuda_device))
     assert torch.equal(z[torch.float16], z[torch.bfloat16])
     zz = z[torch.float16].double().cpu()
-    assert np.abs(zz.numpy() - CI.start_noise(77, n)).max() <= 1e-5
+    assert np.abs(zz.numpy() - CN.normals(77, CN.START, 0, n)).max() <= 1e-5
     assert abs(zz.mean().item()) < 5 / n ** 0.5 and abs(zz.var().item() - 1) < 0.02
 
 

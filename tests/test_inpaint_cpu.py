@@ -1,9 +1,8 @@
-"""Inpainting requests (`Request.repaint_mask`) without a GPU: validation, the blend's noise stream against the other
-streams of a seed, the pixel-to-latent mask reduction, inpainting requests of every sampler kind next to plain and
-image-to-image requests in `sample_requests` and `SamplingEngine` against each request's own sampler with
-`diffusion.q_sample` drawing the seeded blend noise, the all-repaint / all-keep edges, the corrector of a first PLMS
-step, and the paste-back of image outputs.  The UNet is the fake of fake_unet.py, the first stage the fake of
-cases_encode.py and the kernels are restated in torch."""
+"""Inpainting requests (`Request.repaint_mask`) without a GPU: validation, the pixel-to-latent mask reduction,
+inpainting requests of every sampler kind next to plain and image-to-image requests in `sample_requests` and
+`SamplingEngine` against each request's own sampler with `diffusion.q_sample` drawing the seeded blend noise, the
+all-repaint / all-keep edges, the corrector of a first PLMS step, and the paste-back of image outputs.  The UNet is the
+fake of fake_unet.py, the first stage the fake of cases_encode.py and the kernels are restated in torch."""
 import os
 import sys
 from contextlib import contextmanager
@@ -15,14 +14,10 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-import cases_ddim as CD  # noqa: E402
-import cases_decode as CDec  # noqa: E402
-import cases_dpm as CPM  # noqa: E402
 import cases_encode as CE  # noqa: E402
 import cases_img2img as CI  # noqa: E402
 import cases_inpaint as CP  # noqa: E402
-from fake_unet import FakeUNet, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
-from instancediffusion_b200 import ops  # noqa: E402
+from fake_unet import FakeUNet, _fresh, _req, torch_kernels  # noqa: E402,F401
 from instancediffusion_b200.ldm.models.diffusion.batched import (  # noqa: E402
     check_requests, keep_mask, sample_requests)
 from instancediffusion_b200.ldm.models.diffusion.ddim import DDIMSampler  # noqa: E402
@@ -39,17 +34,6 @@ S = 10
 def diffusion():
     from instancediffusion_b200.ldm.models.diffusion.ldm import LatentDiffusion
     return LatentDiffusion(linear_start=0.00085, linear_end=0.012, timesteps=1000)
-
-
-@pytest.fixture
-def torch_kernels(monkeypatch):
-    monkeypatch.setattr(ops, "plms_update", _plms_update)
-    monkeypatch.setattr(ops, "latent_mean", _latent_mean)
-    monkeypatch.setattr(ops, "ddim_update", CD.ddim_update)
-    monkeypatch.setattr(ops, "noise_latent", CI.noise_latent)
-    monkeypatch.setattr(ops, "dpmpp2m_update", CPM.dpmpp2m_update)
-    monkeypatch.setattr(ops, "decode_to_image", CDec.decode_to_image)
-    monkeypatch.setattr(ops, "inpaint_blend", CP.inpaint_blend)
 
 
 def _x_init(seed, b=1):
@@ -120,7 +104,7 @@ def _engine(diffusion, reqs, arrivals=None, **kw):
 
 
 # ------------------------------------------------------------------------------------------------
-# validation, the mask reduction, the noise stream
+# validation and the mask reduction
 # ------------------------------------------------------------------------------------------------
 def test_check_requests_repaint_mask():
     ok = _req(1, S)
@@ -168,28 +152,6 @@ def test_keep_mask_reduction():
         assert keep[b, y, x] == int(not m[b, 8 * y:8 * y + 8, 8 * x:8 * x + 8].any())
     box = keep_mask(_box(box=(8, 17, 0, 8)))  # rows 8..16: latent rows 1 and 2 (one pixel of row 2)
     assert box[0, :, 0].tolist() == [1, 0, 0, 1, 1, 1, 1, 1] + [1] * 56 and int(box[0, :, 1:].sum()) == 64 * 63
-
-
-def test_blend_noise_stream():
-    """Counter word 3 = 3: disjoint from the DDIM eta (0), start (1) and encoder posterior (2) streams of the same seed;
-    element i is a function of (seed, t, i) alone."""
-    n = 4 * 4096 + 3
-    for seed in (0, 7, 2 ** 63 + 1, 2 ** 64 - 1):
-        for t in (0, 1, 981):
-            z = CP.blend_noise(seed, t, n)
-            assert not np.isin(z, CD.ddim_noise(seed, t, n)).any()
-            assert not np.isin(z, CI.start_noise(seed, n)).any()
-            assert not np.isin(z, CE.posterior_noise(seed, t, n)).any()
-            assert np.array_equal(CP.blend_noise(seed, t, 10), z[:10])
-        assert not np.isin(CP.blend_noise(seed, 1, n), CP.blend_noise(seed, 2, n)).any()
-        c = np.arange(3, dtype=np.uint64)
-        words = CD.philox4x32([c, np.zeros(3, np.uint32), np.full(3, 21, np.uint32), np.full(3, 3, np.uint32)],
-                              [np.uint32(seed & 0xFFFFFFFF), np.uint32(seed >> 32)])
-        u = (words.astype(np.float64) + 0.5) * 2.0 ** -32
-        r = np.sqrt(-2 * np.log(u[0]))
-        assert np.allclose(CP.blend_noise(seed, 21, 12)[0::4], r * np.cos(2 * np.pi * u[1]), rtol=0, atol=1e-12)
-    z = CP.blend_noise(123, 500, 200000)
-    assert abs(z.mean()) < 0.01 and abs(z.std() - 1) < 0.01
 
 
 # ------------------------------------------------------------------------------------------------

@@ -18,6 +18,7 @@ sys.path.insert(0, HERE)
 import cases  # noqa: E402
 import cases_encode as CE  # noqa: E402
 import cases_inpaint as CP  # noqa: E402
+import cases_noise as CN  # noqa: E402
 from test_ddim_gpu import DDIM_GOLDEN_TOL, DDIM_LATENT_TOL, _rel, diffusion, unet  # noqa: E402,F401 (module fixtures)
 from test_engine_gpu import _drive  # noqa: E402
 from test_requests_gpu import _fresh, _reset  # noqa: E402
@@ -90,7 +91,7 @@ def test_inpaint_blend_noise_matches_the_cpu_mirror(cuda_device):
     ops.inpaint_blend([torch.zeros(shape, device=cuda_device)], [z], torch.zeros(shape, device=cuda_device),
                       torch.ones((1, 128, 128), dtype=torch.uint8, device=cuda_device), (0.0, 1.0), 77, 501)
     zz = z.double().cpu().reshape(-1).numpy()
-    assert np.abs(zz - CP.blend_noise(77, 501, n)).max() <= 1e-5
+    assert np.abs(zz - CN.normals(77, CN.INPAINT, 501, n)).max() <= 1e-5
     assert abs(zz.mean()) < 5 / n ** 0.5 and abs(zz.var() - 1) < 0.02
 
 

@@ -10,8 +10,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from fake_unet import AGEN, FakeUNet, _alone, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
-from instancediffusion_b200 import ops  # noqa: E402
+from fake_unet import AGEN, FakeUNet, _alone, _fresh, _req, torch_kernels  # noqa: E402,F401
 from instancediffusion_b200.ldm.models.diffusion.batched import (  # noqa: E402
     Request, RequestPlan, check_requests, plan_chunks, plan_step, sample_requests, schedule_steps)
 from instancediffusion_b200.ldm.modules.diffusionmodules.util import make_ddim_timesteps  # noqa: E402
@@ -105,13 +104,11 @@ def test_validation_errors():
 
 
 @pytest.mark.parametrize("S", [10, 11])
-def test_sample_requests_forwards_and_latents(monkeypatch, S):
+def test_sample_requests_forwards_and_latents(torch_kernels, S):
     """Plain, mis 0.36, mis 1.0 and no-alpha-schedule requests in one run on the fake UNet, its fusers at 0.5: every
     forward (images, timesteps, fuser scales and conv flags per input, the corrector forwards of step 0 after the
     predictor's), the model's conv and fuser scale afterwards, and each latent against the request's own sampler."""
     from instancediffusion_b200.ldm.models.diffusion.ldm import LatentDiffusion
-    monkeypatch.setattr(ops, "plms_update", _plms_update)
-    monkeypatch.setattr(ops, "latent_mean", _latent_mean)
     diffusion = LatentDiffusion(linear_start=0.00085, linear_end=0.012, timesteps=1000)
     ones = partial(alpha_generator, type=[1.0, 0.0, 0.0])
     reqs = [_req(31, S), _req(32, S, n=2, mis=0.36), _req(33, S, n=1, mis=1.0, alpha=ones), _req(34, S, alpha=None)]

@@ -13,12 +13,8 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-import cases_ddim as CD  # noqa: E402
-import cases_dpm as CP  # noqa: E402
-import cases_img2img as CI  # noqa: E402
-from fake_unet import AGEN, FakeUNet, _fresh, _latent_mean, _plms_update, _req  # noqa: E402
+from fake_unet import AGEN, FakeUNet, _fresh, _req, torch_kernels  # noqa: E402,F401
 from test_img2img_cpu import _i2i  # noqa: E402
-from instancediffusion_b200 import ops  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion.ddim import DDIMSampler  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion.dpm_solver import DPMSolverSampler  # noqa: E402
 from instancediffusion_b200.ldm.models.diffusion.plms import PLMSSampler  # noqa: E402
@@ -26,20 +22,13 @@ from instancediffusion_b200.ldm.models.diffusion.plms_instance import PLMSSample
 from instancediffusion_b200.ldm.modules.diffusionmodules.util import make_ddim_timesteps  # noqa: E402
 from instancediffusion_b200.utils.model import set_alpha_scale  # noqa: E402
 
+pytestmark = pytest.mark.usefixtures("torch_kernels")
+
 
 @pytest.fixture
 def diffusion():
     from instancediffusion_b200.ldm.models.diffusion.ldm import LatentDiffusion
     return LatentDiffusion(linear_start=0.00085, linear_end=0.012, timesteps=1000)
-
-
-@pytest.fixture(autouse=True)
-def torch_kernels(monkeypatch):
-    monkeypatch.setattr(ops, "plms_update", _plms_update)
-    monkeypatch.setattr(ops, "latent_mean", _latent_mean)
-    monkeypatch.setattr(ops, "ddim_update", CD.ddim_update)
-    monkeypatch.setattr(ops, "noise_latent", CI.noise_latent)
-    monkeypatch.setattr(ops, "dpmpp2m_update", CP.dpmpp2m_update)
 
 
 class LoggingUNet(FakeUNet):

@@ -7,7 +7,7 @@ UNet of tests/cases.py UNET_CASE.  Needs a reference checkout ($IDIFF_REF, see o
 Each case is the strength-1 inpainting request of the project's drivers: input["x"] is x_init noised at the first
 timestep with the image-to-image start noise (tests/cases_img2img.py), mask is the latent keep mask of the case's pixel
 box and x0 = x_init.  The reference diffusion's q_sample is wrapped to pass its own `noise=` argument the seeded blend
-stream (tests/cases_inpaint.py blend_noise at the step's timestep) in place of torch.randn_like; the sampler loops are
+stream (tests/cases_noise.py INPAINT at the step's timestep) in place of torch.randn_like; the sampler loops are
 not edited.  Only the latents are written.
 """
 from __future__ import annotations
@@ -27,6 +27,7 @@ GOLDEN = os.path.join(REPO, "tests", "golden")
 import cases  # noqa: E402
 import cases_img2img as CI  # noqa: E402
 import cases_inpaint as CP  # noqa: E402
+import cases_noise as CN  # noqa: E402
 from oracle import ref_harness, torch_oracle  # noqa: E402
 from instancediffusion_b200 import synthetic  # noqa: E402
 
@@ -62,7 +63,7 @@ def main():
 
         def seeded(x_start, t, seed=sc["seed"]):
             tt = int(t.reshape(-1)[0])
-            z = torch.from_numpy(CP.blend_noise(seed, tt, x_start.numel())).view_as(x_start).float()
+            z = torch.from_numpy(CN.normals(seed, CN.INPAINT, tt, x_start.numel())).view_as(x_start).float()
             return q_sample(x_start, t, noise=z)
         diffusion.q_sample = seeded
         agen = partial(torch_oracle.alpha_schedule, alpha_type=sc["alpha_type"])
